@@ -93,6 +93,58 @@ def opaque_stack_scene(layers: int, grid: int, views: int, h: int, w: int, seed:
     return _with_extra(sc, means, scales, opac, g)
 
 
+def _at_pixels(u, v, z, h: int, w: int):
+    """World points (view 0, identity camera) whose centres project to pixel coordinates (u, v) at depth z -- the
+    inverse of the rasterizer's ((ndc + 1) * W - 1) / 2."""
+    x = ((2 * u + 1) / w - 1) * TANFOV * z
+    y = ((2 * v + 1) / h - 1) * TANFOV * z
+    return torch.stack([x, y, z], -1)
+
+
+def edge_straddle_scene(P: int, n_edge: int, views: int, h: int, w: int, seed: int = 0) -> Scene:
+    """P ordinary splats plus n_edge whose centres lie within 2 pixels of the last column or the last row (half of them
+    each; some beyond the frame), with footprints of 0.5-3 pixels: they reach the pixels of a partial warp column (8
+    wide) or row (4 high) of the backward compositor, and the last tile row and column of the frame."""
+    sc = make_scene(P, views, h, w, seed=seed)
+    g = torch.Generator().manual_seed(seed + 4000)
+    z = _U(g, 2.0, 8.0, n_edge)
+    right = torch.arange(n_edge) % 2 == 0
+    along_u, along_v = _U(g, -1.0, w, n_edge), _U(g, -1.0, h, n_edge)
+    u = torch.where(right, (w - 1) + _U(g, -2.0, 2.0, n_edge), along_u)
+    v = torch.where(right, along_v, (h - 1) + _U(g, -2.0, 2.0, n_edge))
+    means = _at_pixels(u, v, z, h, w)
+    f_px = w / (2 * TANFOV)
+    sigma = torch.exp(_U(g, math.log(0.5), math.log(3.0), n_edge)) * z / f_px
+    scales = sigma[:, None] * torch.exp(_U(g, -0.3, 0.3, n_edge, 3))
+    opac = _U(g, 0.2, 0.95, n_edge)
+    return _with_extra(sc, means, scales, opac, g)
+
+
+def long_list_scene(n: int, views: int, h: int, w: int, box=None, n_sparse: int = 0, sparse_box=None,
+                    seed: int = 0) -> Scene:
+    """n faint, nearly pixel-sized splats (opacity 0.01-0.03, sigma about 0.2 px before the 0.3 px^2 dilation) spread
+    over the pixel box (u0, v0, u1, v1) of view 0 at depths 3-8 -- all of them in one 16 x 16 tile when the box is
+    inside one: that tile's list is n long, each pixel is reached by about n * 3 / (box area) of them, and its
+    transmittance stays far above 1e-4, so its last contributor sits near the end of the list.  Plus n_sparse
+    ordinary-sized ones (0.5-2 px, opacity 0.1-0.8) in `sparse_box`, so that the tiles outside both boxes stay empty."""
+    sc = make_scene(0, views, h, w, seed=seed)
+    g = torch.Generator().manual_seed(seed + 5000)
+    f_px = w / (2 * TANFOV)
+
+    def cloud(k, bx, sig_lo, sig_hi, o_lo, o_hi):
+        u0, v0, u1, v1 = bx
+        z = _U(g, 3.0, 8.0, k)
+        means = _at_pixels(_U(g, u0, u1, k), _U(g, v0, v1, k), z, h, w)
+        sigma = torch.exp(_U(g, math.log(sig_lo), math.log(sig_hi), k)) * z / f_px
+        return means, sigma[:, None] * torch.exp(_U(g, -0.2, 0.2, k, 3)), _U(g, o_lo, o_hi, k)
+
+    m, s, o = cloud(n, box or (0.0, 0.0, w - 1.0, h - 1.0), 0.15, 0.3, 0.01, 0.03)
+    if n_sparse:
+        m2, s2, o2 = cloud(n_sparse, sparse_box, 0.5, 2.0, 0.1, 0.8)
+        m, s, o = torch.cat([m, m2]), torch.cat([s, s2]), torch.cat([o, o2])
+    return _with_extra(sc, m, s, o, g)
+
+
 def stacked_views_cameras(sc: Scene, views_per_chunk: int = 8, step: float = 8.0) -> Scene:
     """sc with view k moved back along the optical axis by step * (k // views_per_chunk): each chunk of views sees the
     cloud at its own range of depths (the depth-stratum boundaries of one chunk do not fit the next)."""

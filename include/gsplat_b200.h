@@ -291,6 +291,30 @@ GS_API int gs_adapter_forward(const GsAdapterConfig *cfg, const GsAdapterInputs 
 GS_API int gs_adapter_backward(const GsAdapterConfig *cfg, const GsAdapterInputs *in, const GsAdapterOutGrads *gout,
                         const GsAdapterInGrads *gin, void *stream);
 
+/*
+ * Photometric training loss = PF3plat's LossMultiSSIM + LossMse (src/loss/loss_multissim.py:45-86, loss_mse.py:35),
+ * forward and backward.  Per image: ssim = the mean over (c, h, w) of the single-scale SSIM map with the zero-padded
+ * 11 x 11 Gaussian window (sigma 1.5) and population covariance, no clipping; mse = the mean of (pred - gt)^2.  Any
+ * height and width >= 1 is legal (the window may be larger than the image).
+ * Device pointers.  predicted / ground_truth: `batch` images, image i at i * stride floats, each (c,h,w) block
+ * contiguous; scratch: gs_photometric_scratch_bytes(cfg) bytes, 8-byte aligned (the backward needs none and ignores
+ * it); out_ssim [batch]; out_mse [batch], required iff with_mse.  The incoming gradients dL_dssim / dL_dmse [batch]
+ * are device arrays (NULL = zero; dL_dmse is read only if with_mse); the gradients dL_dpredicted / dL_dground_truth are
+ * written contiguous [batch, c, h, w] (NULL = not wanted).  Deterministic (no atomics), no host synchronisation.
+ */
+typedef struct GsLossConfig {
+    int32_t batch, channels, height, width;
+    int64_t pred_stride, gt_stride; /* floats between consecutive images (ignored when batch == 1) */
+    int32_t with_mse, reserved_;    /* with_mse: 0 or 1 */
+} GsLossConfig;
+
+GS_API int64_t gs_photometric_scratch_bytes(const GsLossConfig *cfg); /* -1 for an invalid config */
+GS_API int gs_photometric_forward(const GsLossConfig *cfg, const float *predicted, const float *ground_truth, void *scratch,
+                                  float *out_ssim, float *out_mse, void *stream);
+GS_API int gs_photometric_backward(const GsLossConfig *cfg, const float *predicted, const float *ground_truth,
+                                   const float *dL_dssim, const float *dL_dmse, float *dL_dpredicted,
+                                   float *dL_dground_truth, void *scratch, void *stream);
+
 /* Per-stage device timings (ms) of the last forward/backward when profiling is enabled; CUDA events on `stream`. */
 enum { GS_STAGE_PREPROCESS = 0,      /* k_preprocess (incl. tile counting) */
        GS_STAGE_BIN_SCAN = 1,        /* k_tile_scan + the forward's one host read-back */

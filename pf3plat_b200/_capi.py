@@ -101,6 +101,11 @@ class GsAdapterInGrads(Structure):
                 ("kinv", c_void_p), ("multiplier", c_void_p)]
 
 
+class GsLossConfig(Structure):
+    _fields_ = [("batch", c_int32), ("channels", c_int32), ("height", c_int32), ("width", c_int32),
+                ("pred_stride", c_int64), ("gt_stride", c_int64), ("with_mse", c_int32), ("reserved_", c_int32)]
+
+
 SYMBOLS = {
     "gs_abi_version": (c_int, []),
     "gs_last_error": (c_char_p, []),
@@ -124,6 +129,10 @@ SYMBOLS = {
     "gs_adapter_forward": (c_int, [POINTER(GsAdapterConfig), POINTER(GsAdapterInputs), POINTER(GsAdapterOutputs), c_void_p]),
     "gs_adapter_backward": (c_int, [POINTER(GsAdapterConfig), POINTER(GsAdapterInputs), POINTER(GsAdapterOutGrads),
                                     POINTER(GsAdapterInGrads), c_void_p]),
+    "gs_photometric_scratch_bytes": (c_int64, [POINTER(GsLossConfig)]),
+    "gs_photometric_forward": (c_int, [POINTER(GsLossConfig), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "gs_photometric_backward": (c_int, [POINTER(GsLossConfig), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                        c_void_p, c_void_p]),
 }
 
 

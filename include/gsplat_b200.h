@@ -315,6 +315,40 @@ GS_API int gs_photometric_backward(const GsLossConfig *cfg, const float *predict
                                    const float *dL_dssim, const float *dL_dmse, float *dL_dpredicted,
                                    float *dL_dground_truth, void *scratch, void *stream);
 
+/*
+ * LPIPS-VGG = the `lpips` package's LPIPS(net="vgg", version="0.1"), spatial=False, as PF3plat's LossLpips
+ * (src/loss/loss_lpips.py:55-59) and compute_lpips (src/evaluation/metrics.py:27-33) call it; forward and input
+ * gradients (the weights are constants).  The weights are an input:
+ *   gs_lpips_weights_create packs, on `stream`, the 13 conv weights [Cout, Cin, 3, 3] and biases [Cout] of VGG16
+ *   features[0:30] (conv1_1 .. conv5_3), the 5 lin weights [C] (relu1_2 .. relu5_3) and the scaling layer's shift[3] and
+ *   scale[3] (all device pointers on the current device) into private device memory; the sources may be freed once the
+ *   stream has run the packing.  gs_lpips_weights_destroy synchronises with the device before it frees.
+ * Inputs in0 / in1: `batch` images [3, height, width], image i at i * stride floats.  height, width >= 16.
+ * workspace: gs_lpips_workspace_bytes(cfg) bytes, 256-byte aligned; with grads != 0 the forward keeps every activation
+ * there for gs_lpips_backward, which must get the same config and workspace.  out [batch] (the package's (N,1,1,1)).
+ * dL_dout [batch] is a device array; dL_din0 / dL_din1 are written contiguous [batch, 3, height, width], NULL = not
+ * wanted (each needs its bit in grads).  Deterministic (no atomics), no host synchronisation.
+ */
+typedef struct GsLpipsWeights GsLpipsWeights;
+
+typedef struct GsLpipsConfig {
+    int32_t batch, height, width;
+    int32_t normalize;              /* 0 or 1: inputs are mapped x -> 2x - 1 first (the package's normalize=True) */
+    int64_t in0_stride, in1_stride; /* floats between consecutive images (ignored when batch == 1) */
+    int32_t grads;                  /* bit 0: dL/din0 will be wanted, bit 1: dL/din1; 0 = forward only */
+    int32_t reserved_;
+} GsLpipsConfig;
+
+GS_API int gs_lpips_weights_create(const float *const *conv_weight /* [13] */, const float *const *conv_bias /* [13] */,
+                                   const float *const *lin /* [5] */, const float *shift, const float *scale, void *stream,
+                                   GsLpipsWeights **out);
+GS_API void gs_lpips_weights_destroy(GsLpipsWeights *weights);
+GS_API int64_t gs_lpips_workspace_bytes(const GsLpipsConfig *cfg); /* -1 for an invalid config */
+GS_API int gs_lpips_forward(const GsLpipsWeights *weights, const GsLpipsConfig *cfg, const float *in0, const float *in1,
+                            void *workspace, float *out, void *stream);
+GS_API int gs_lpips_backward(const GsLpipsWeights *weights, const GsLpipsConfig *cfg, const float *dL_dout,
+                             void *workspace, float *dL_din0, float *dL_din1, void *stream);
+
 /* Per-stage device timings (ms) of the last forward/backward when profiling is enabled; CUDA events on `stream`. */
 enum { GS_STAGE_PREPROCESS = 0,      /* k_preprocess (incl. tile counting) */
        GS_STAGE_BIN_SCAN = 1,        /* k_tile_scan + the forward's one host read-back */

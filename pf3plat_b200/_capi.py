@@ -106,6 +106,11 @@ class GsLossConfig(Structure):
                 ("pred_stride", c_int64), ("gt_stride", c_int64), ("with_mse", c_int32), ("reserved_", c_int32)]
 
 
+class GsLpipsConfig(Structure):
+    _fields_ = [("batch", c_int32), ("height", c_int32), ("width", c_int32), ("normalize", c_int32),
+                ("in0_stride", c_int64), ("in1_stride", c_int64), ("grads", c_int32), ("reserved_", c_int32)]
+
+
 SYMBOLS = {
     "gs_abi_version": (c_int, []),
     "gs_last_error": (c_char_p, []),
@@ -133,6 +138,12 @@ SYMBOLS = {
     "gs_photometric_forward": (c_int, [POINTER(GsLossConfig), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "gs_photometric_backward": (c_int, [POINTER(GsLossConfig), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                         c_void_p, c_void_p]),
+    "gs_lpips_weights_create": (c_int, [POINTER(c_void_p), POINTER(c_void_p), POINTER(c_void_p), c_void_p, c_void_p,
+                                        c_void_p, POINTER(c_void_p)]),
+    "gs_lpips_weights_destroy": (None, [c_void_p]),
+    "gs_lpips_workspace_bytes": (c_int64, [POINTER(GsLpipsConfig)]),
+    "gs_lpips_forward": (c_int, [c_void_p, POINTER(GsLpipsConfig), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "gs_lpips_backward": (c_int, [c_void_p, POINTER(GsLpipsConfig), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
 }
 
 

@@ -6,8 +6,8 @@ photometric terms:
                name: zero-padded 11x11 Gaussian window, sigma 1.5, population covariance, no clipping);
   * `photometric_loss` -- `LossMse` (loss_mse.py:35) + `LossMultiSSIM` (loss_multissim.py:41-43) in one forward and one
                backward kernel, each term already weighted as the reference logs it (`loss/mse`, `loss/MultiSSIM`).
-Both are differentiable with respect to both images.  LPIPS (pretrained VGG weights) and the pose loss (encoder side)
-are not here.  Inputs must be float32 CUDA tensors; there is no CPU fallback.
+Both are differentiable with respect to both images.  LPIPS is `pf3plat_b200.lpips.LPIPS`; the pose loss (encoder side)
+is not here.  Inputs must be float32 CUDA tensors; there is no CPU fallback.
 """
 from __future__ import annotations
 

@@ -1,14 +1,17 @@
 """Image metrics of the evaluation path (SURVEY.md section 8(f).4).
 
-`compute_psnr` and `compute_ssim` have the signatures and semantics of the reference's
-(PF3plat's src/evaluation/metrics.py:11-19, :38-54) and run on the device (gs_metrics.cu); the reference's
-SSIM loops over images on the CPU through scikit-image.  (`compute_lpips` needs the pretrained VGG weights of the
-`lpips` package -- no network here -- and is out of scope.)"""
+`compute_psnr`, `compute_lpips` and `compute_ssim` have the signatures and semantics of the reference's
+(PF3plat's src/evaluation/metrics.py:11-19, :27-33, :38-54) and run on the device (gs_metrics.cu, gs_lpips.cu); the
+reference's SSIM loops over images on the CPU through scikit-image.  `compute_lpips` takes the pretrained VGG weights
+of the installed `lpips` package, as the reference does (pf3plat_b200.lpips.LPIPS)."""
 from __future__ import annotations
+
+import functools
 
 import torch
 
 from . import _capi
+from .lpips import LPIPS
 
 
 @torch.no_grad()
@@ -29,6 +32,19 @@ def compute_psnr(ground_truth: torch.Tensor, predicted: torch.Tensor) -> torch.T
         _capi.check(L.gs_psnr(gt.data_ptr(), pr.data_ptr(), b, n, scratch.data_ptr(), out.data_ptr(),
                               torch.cuda.current_stream(pr.device).cuda_stream))
     return out
+
+
+@functools.cache
+def get_lpips(device: torch.device) -> LPIPS:
+    """One LPIPS-VGG module per device (metrics.py:22-24)."""
+    return LPIPS(net="vgg").to(device)
+
+
+@torch.no_grad()
+def compute_lpips(ground_truth: torch.Tensor, predicted: torch.Tensor) -> torch.Tensor:
+    """(batch, 3, height, width) x 2 -> (batch,) LPIPS-VGG distance, inputs in [0, 1] (normalize=True)."""
+    value = get_lpips(predicted.device).forward(ground_truth, predicted, normalize=True)
+    return value[:, 0, 0, 0]
 
 
 @torch.no_grad()

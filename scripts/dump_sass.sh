@@ -15,3 +15,4 @@ dump gs_composite_bwd "k_composite_bwd_v1ILb0" r2_k_composite_bwd_v1
 dump gs_binning "k_stratum_rank_sort" r2_k_stratum_rank_sort
 dump gs_preprocess "k_sh_colour" r2_k_sh_colour
 # (the per-kernel mnemonic histogram profiles/r2_sass_mnemonics.txt is written by scripts/sass_mnemonics.py)
+dump gs_lpips "k_conv3x3" lpips_k_conv3x3   # tensor cores: HMMA.1688.F32.TF32

@@ -34,7 +34,7 @@
 extern "C" {
 #endif
 
-#define GS_ABI_VERSION 1
+#define GS_ABI_VERSION 2
 
 #if defined(__GNUC__)
 #define GS_API __attribute__((visibility("default")))
@@ -139,6 +139,11 @@ typedef struct GsInGrads {
     float *dL_dscales;     /* device [S,P,3] */
     float *dL_drotations;  /* device [S,P,4] */
     float *dL_dcov3D;      /* device [S,P,6] */
+    /* device [V,4]: dL/d(viewmatrix flat entries 2, 6, 10, 14), the z column of the transposed view matrix, through the
+     * fused depth channel only (z = that column . (view_scale * mean, 1)), as render_depth_cuda's fake colour carries it
+     * (cuda_splatting.py:239-242).  Colour, projection and culling give the cameras no gradient.  NULL = not wanted;
+     * needs GS_FLAG_DEPTH.  Written, not accumulated; zeros when dL_ddepth is NULL. */
+    float *dL_dviewmatrix_z;
 } GsInGrads;
 
 /* Counters of the last forward on a context (host-visible after the call returns). */

@@ -12,7 +12,7 @@ from ctypes import POINTER, Structure, c_char_p, c_float, c_int, c_int32, c_int6
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "csrc", "libgsplat_b200.so")
-ABI_VERSION = 1
+ABI_VERSION = 2
 
 GS_FLAG_DEPTH = 1
 GS_FLAG_PREFILTERED = 2
@@ -64,7 +64,7 @@ class GsOutGrads(Structure):
 class GsInGrads(Structure):
     _fields_ = [("dL_dmeans3D", c_void_p), ("dL_dmeans2D", c_void_p), ("dL_dshs", c_void_p), ("dL_dcolors", c_void_p),
                 ("dL_dopacities", c_void_p), ("dL_dscales", c_void_p), ("dL_drotations", c_void_p),
-                ("dL_dcov3D", c_void_p)]
+                ("dL_dcov3D", c_void_p), ("dL_dviewmatrix_z", c_void_p)]
 
 
 class GsStats(Structure):

@@ -61,7 +61,12 @@ class ViewBatch:
 
 
 def make_view_batch(extrinsics, intrinsics, near, far, scale_invariant: bool = True) -> ViewBatch:
-    """cuda_splatting.py:64-87 for all views at once (no per-view `.item()` host syncs)."""
+    """cuda_splatting.py:64-87 for all views at once (no per-view `.item()` host syncs).
+
+    On CUDA tensors whose extrinsics require grad, `viewmatrix` is differentiable w.r.t. them: its values are the
+    kernel's, its gradient that of the view matrix built in torch.  This is what lets the fused depth channel carry
+    render_depth_cuda's camera gradient (cuda_splatting.py:239-242).  `projmatrix`, `campos` and `tanfov` stay
+    detached, and `near` / `far` get no gradient."""
     if extrinsics.is_cuda:
         return _make_view_batch_cuda(extrinsics, intrinsics, near, far, scale_invariant)
     if scale_invariant:
@@ -100,4 +105,15 @@ def _make_view_batch_cuda(extrinsics, intrinsics, near, far, scale_invariant: bo
         _capi.check(_capi.lib().gs_view_batch(B, int(bool(scale_invariant)), p(ext), p(intr), p(nr), p(fr), p(view), p(proj),
                                               p(campos), p(tanfov), p(scale),
                                               ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)))
+    if extrinsics.requires_grad and torch.is_grad_enabled():
+        # The kernel's values (plus exact zeros) with the gradient of a torch expression of the view matrix.  The
+        # expression rescales the translation of extrinsics^-1 rather than that of the extrinsics
+        # (cuda_splatting.py:64-86).  Both are equal while the bottom row is (0, 0, 0, 1), but only this one differentiates
+        # like render_depth_cuda's z = (extrinsics^-1 @ mean).z once the depth is multiplied back by near, in every
+        # entry, the bottom row's included.
+        w2c = torch.linalg.inv(extrinsics).clone()
+        if scale_invariant:
+            w2c[..., :3, 3] = w2c[..., :3, 3] * (1.0 / near.detach().to(dev, w2c.dtype))[:, None]
+        vt = w2c.transpose(-1, -2)
+        view = view + (vt - vt.detach()).to(view.dtype)
     return ViewBatch(view, proj, campos, tanfov, scale)

@@ -782,7 +782,16 @@ extern "C" int gs_backward(GsContext *ctx, const GsConfig *cfg, const GsInputs *
     if (saved->P != c.P || saved->V != c.V || saved->S != c.S || saved->H != c.H || saved->W != c.W)
         return gs_set_error(GS_ERR_INVALID, "saved state does not match the configuration");
     c.flags = saved->flags;
+    if (gin->dL_dviewmatrix_z && !(c.flags & GS_FLAG_DEPTH))
+        return gs_set_error(GS_ERR_INVALID, "dL_dviewmatrix_z needs a forward with GS_FLAG_DEPTH");
     const DevInputs di = make_dev_inputs(in);
+    // the view-matrix gradient is written: zero it, then the kernels accumulate into it (nothing when there is no
+    // incoming depth gradient: it stays zero and the default kernels run)
+    GsInGrads g = *gin;
+    if (g.dL_dviewmatrix_z) {
+        GS_CUDA_OK(cudaMemsetAsync(g.dL_dviewmatrix_z, 0, (size_t)c.V * 4 * sizeof(float), st));
+        if (!gout->dL_ddepth) g.dL_dviewmatrix_z = nullptr;
+    }
     const size_t n = (size_t)c.V * c.P;
     if (n == 0) return GS_OK;
 
@@ -797,7 +806,7 @@ extern "C" int gs_backward(GsContext *ctx, const GsConfig *cfg, const GsInputs *
     }
     {
         StageTimer t(ctx, GS_STAGE_PREPROCESS_BWD, st);
-        rc = launch_preprocess_bwd(c, di, *saved, acc, *gin, st, (cfg->tuning & GS_TUNE_PBWD_2PHASE) ? 1 : 0);
+        rc = launch_preprocess_bwd(c, di, *saved, acc, g, st, (cfg->tuning & GS_TUNE_PBWD_2PHASE) ? 1 : 0);
         if (rc != GS_OK) return rc;
     }
     ctx->stats.kernel_launches += 2;  // k_composite_bwd, k_preprocess_bwd

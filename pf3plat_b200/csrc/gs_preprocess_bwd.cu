@@ -77,7 +77,29 @@ __device__ __forceinline__ void sh_backward_channel(int deg, const float *sh, fl
     ddz += dz_ * g;
 }
 
-template <bool HAS_SH, int MINB>
+// dL/d(view matrix entries 2, 6, 10, 14) of one view += the warp's sum of (gz * m, gz): a butterfly over the 32 lanes,
+// then one RED per component from lane 0.  Every lane of the warp must call it for the same view (inactive lanes with
+// zeros); the calls may sit at different points of the code (shfl.sync on sm_70 and later).
+__device__ __forceinline__ void red_view_z_grad(float *dst, float a, float b, float c, float d) {
+#pragma unroll
+    for (int off = 16; off > 0; off >>= 1) {
+        a += __shfl_xor_sync(0xffffffffu, a, off);
+        b += __shfl_xor_sync(0xffffffffu, b, off);
+        c += __shfl_xor_sync(0xffffffffu, c, off);
+        d += __shfl_xor_sync(0xffffffffu, d, off);
+    }
+    if ((threadIdx.x & 31) == 0) {
+        atomicAdd(dst + 0, a);
+        atomicAdd(dst + 1, b);
+        atomicAdd(dst + 2, c);
+        atomicAdd(dst + 3, d);
+    }
+}
+
+// VIEW_Z: also write g.dL_dviewmatrix_z, the depth channel's gradient w.r.t. the z column of each view matrix
+// (z = view[2] m.x + view[6] m.y + view[10] m.z + view[14], m the view-scaled mean).  The default instantiations
+// (VIEW_Z = false) are the kernels without it, instruction for instruction.
+template <bool HAS_SH, int MINB, bool VIEW_Z = false>
 __global__ void __launch_bounds__(PB_THREADS, MINB)
 k_preprocess_bwd(const DevCfg c, const DevInputs in, const uint8_t *__restrict__ meta, const float *__restrict__ acc,
                     const GsInGrads g) {
@@ -145,11 +167,15 @@ k_preprocess_bwd(const DevCfg c, const DevInputs in, const uint8_t *__restrict__
             load_view_cams(c, v, min(GS_CAM_CHUNK, c.VPS - vi), sm->cams);
             __syncthreads();
         }
-        if (!active) continue;
+        if (!active) {
+            if (VIEW_Z) red_view_z_grad(g.dL_dviewmatrix_z + (size_t)v * 4, 0.f, 0.f, 0.f, 0.f);
+            continue;
+        }
         const ViewCam &cam = sm->cams[vi % GS_CAM_CHUNK];
         const size_t o = (size_t)v * c.P + i;
         const uint32_t mb = meta[o];
         float m2d[2] = {0.f, 0.f}, gcol[3] = {0.f, 0.f, 0.f};
+        if (VIEW_Z && !(mb & GS_META_VISIBLE)) red_view_z_grad(g.dL_dviewmatrix_z + (size_t)v * 4, 0.f, 0.f, 0.f, 0.f);
         if (mb & GS_META_VISIBLE) {
             const float *a = acc + o * GS_ACC_STRIDE;
             gcol[0] = a[0]; gcol[1] = a[1]; gcol[2] = a[2];
@@ -222,6 +248,7 @@ k_preprocess_bwd(const DevCfg c, const DevInputs in, const uint8_t *__restrict__
             gm[0] += cam.view[2] * gz;
             gm[1] += cam.view[6] * gz;
             gm[2] += cam.view[10] * gz;
+            if (VIEW_Z) red_view_z_grad(g.dL_dviewmatrix_z + (size_t)v * 4, gz * m.x, gz * m.y, gz * m.z, gz);
             // ---- colour -> SH coefficients and mean (view direction) ----
             if (HAS_SH) {
                 const float d[3] = {m.x - cam.campos[0], m.y - cam.campos[1], m.z - cam.campos[2]};
@@ -345,7 +372,7 @@ k_preprocess_bwd(const DevCfg c, const DevInputs in, const uint8_t *__restrict__
 // camera / direction / basis work is redone per phase), and slower.  The single-pass kernel stays the default.
 constexpr int PB2_MIN_CTAS = 6;
 
-template <bool HAS_SH>
+template <bool HAS_SH, bool VIEW_Z = false>
 __global__ void __launch_bounds__(PB_THREADS, PB2_MIN_CTAS)
 k_preprocess_bwd_2phase(const DevCfg c, const DevInputs in, const uint8_t *__restrict__ meta, const float *__restrict__ acc,
                  const GsInGrads g) {
@@ -422,11 +449,15 @@ k_preprocess_bwd_2phase(const DevCfg c, const DevInputs in, const uint8_t *__res
                 load_view_cams(c, v, min(GS_CAM_CHUNK, c.VPS - vi), sm->cams);
                 __syncthreads();
             }
-            if (!active) continue;
+            if (!active) {
+                if (VIEW_Z) red_view_z_grad(g.dL_dviewmatrix_z + (size_t)v * 4, 0.f, 0.f, 0.f, 0.f);
+                continue;
+            }
             const ViewCam &cam = sm->cams[vi % GS_CAM_CHUNK];
             const size_t o = (size_t)v * c.P + i;
             const uint32_t mb = meta[o];
             float m2d[2] = {0.f, 0.f}, gcol[3] = {0.f, 0.f, 0.f};
+            if (VIEW_Z && !(mb & GS_META_VISIBLE)) red_view_z_grad(g.dL_dviewmatrix_z + (size_t)v * 4, 0.f, 0.f, 0.f, 0.f);
             if (mb & GS_META_VISIBLE) {
                 const float *a = acc + o * GS_ACC_STRIDE;
                 gcol[0] = a[0]; gcol[1] = a[1]; gcol[2] = a[2];
@@ -499,6 +530,7 @@ k_preprocess_bwd_2phase(const DevCfg c, const DevInputs in, const uint8_t *__res
                 gm[0] += cam.view[2] * gz;
                 gm[1] += cam.view[6] * gz;
                 gm[2] += cam.view[10] * gz;
+                if (VIEW_Z) red_view_z_grad(g.dL_dviewmatrix_z + (size_t)v * 4, gz * m.x, gz * m.y, gz * m.z, gz);
 #pragma unroll
                 for (int k = 0; k < 3; k++) gmean[k] += s * gm[k];
             }
@@ -622,27 +654,35 @@ k_preprocess_bwd_2phase(const DevCfg c, const DevInputs in, const uint8_t *__res
     }
 }
 
-}  // namespace
-
-int launch_preprocess_bwd(const DevCfg &c, const DevInputs &in, const GsSaved &s, const float *grad_acc,
-                          const GsInGrads &g, cudaStream_t st, int variant) {
-    if (c.P == 0) return GS_OK;
+template <bool VIEW_Z>
+int launch_preprocess_bwd_t(const DevCfg &c, const DevInputs &in, const GsSaved &s, const float *grad_acc,
+                            const GsInGrads &g, cudaStream_t st, int variant) {
     dim3 grid((c.P + PB_THREADS - 1) / PB_THREADS, c.S);
     if (variant != 1) {  // single pass over the views (default)
         if (in.shs) {
             size_t smem = PB_SMEM_HDR + (size_t)PB_THREADS * c.M * 12;
-            GS_CUDA_OK(cudaFuncSetAttribute(k_preprocess_bwd<true, PB_MIN_CTAS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-            k_preprocess_bwd<true, PB_MIN_CTAS><<<grid, PB_THREADS, smem, st>>>(c, in, s.meta, grad_acc, g);
+            GS_CUDA_OK(cudaFuncSetAttribute(k_preprocess_bwd<true, PB_MIN_CTAS, VIEW_Z>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            k_preprocess_bwd<true, PB_MIN_CTAS, VIEW_Z><<<grid, PB_THREADS, smem, st>>>(c, in, s.meta, grad_acc, g);
         } else {
-            k_preprocess_bwd<false, PB_MIN_CTAS><<<grid, PB_THREADS, PB_SMEM_HDR, st>>>(c, in, s.meta, grad_acc, g);
+            k_preprocess_bwd<false, PB_MIN_CTAS, VIEW_Z><<<grid, PB_THREADS, PB_SMEM_HDR, st>>>(c, in, s.meta, grad_acc, g);
         }
     } else if (in.shs) {
         size_t smem = PB_SMEM_HDR + (size_t)PB_THREADS * (c.M <= PB_SH_EVAL ? c.M * 3 : PB_SH_EVAL * 3 + 1) * 4;
-        GS_CUDA_OK(cudaFuncSetAttribute(k_preprocess_bwd_2phase<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        k_preprocess_bwd_2phase<true><<<grid, PB_THREADS, smem, st>>>(c, in, s.meta, grad_acc, g);
+        GS_CUDA_OK(cudaFuncSetAttribute(k_preprocess_bwd_2phase<true, VIEW_Z>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        k_preprocess_bwd_2phase<true, VIEW_Z><<<grid, PB_THREADS, smem, st>>>(c, in, s.meta, grad_acc, g);
     } else {
-        k_preprocess_bwd_2phase<false><<<grid, PB_THREADS, PB_SMEM_HDR, st>>>(c, in, s.meta, grad_acc, g);
+        k_preprocess_bwd_2phase<false, VIEW_Z><<<grid, PB_THREADS, PB_SMEM_HDR, st>>>(c, in, s.meta, grad_acc, g);
     }
     GS_CUDA_OK(cudaGetLastError());
     return GS_OK;
+}
+
+}  // namespace
+
+// g.dL_dviewmatrix_z non-NULL selects the VIEW_Z kernels; the caller has zeroed it (the kernels accumulate into it).
+int launch_preprocess_bwd(const DevCfg &c, const DevInputs &in, const GsSaved &s, const float *grad_acc,
+                          const GsInGrads &g, cudaStream_t st, int variant) {
+    if (c.P == 0) return GS_OK;
+    return g.dL_dviewmatrix_z ? launch_preprocess_bwd_t<true>(c, in, s, grad_acc, g, st, variant)
+                              : launch_preprocess_bwd_t<false>(c, in, s, grad_acc, g, st, variant);
 }

@@ -191,10 +191,20 @@ def _make_config(bs: BatchSettings, S: int, P: int, M: int, keep: list) -> GsCon
 
 
 class _RasterizeBatch(torch.autograd.Function):
-    """The reference's _RasterizeGaussians (SURVEY.md section 3.4), batched over views."""
+    """The reference's _RasterizeGaussians (SURVEY.md section 3.4), batched over views.
+
+    `viewmatrix` is bs.viewmatrix, handed in as a tensor input so that autograd can route a gradient to it.  It gets
+    one only through the fused depth channel (bs.with_depth), as the reference's depth pass gives its cameras one
+    through its fake colour z (cuda_splatting.py:239-242): dL/dviewmatrix is zero outside the z column, and None when
+    the depth is not part of the loss.  Colour, projection and culling give the cameras no gradient, as in the
+    reference op."""
 
     @staticmethod
-    def forward(ctx, means3D, means2D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp, bs: BatchSettings):
+    def forward(ctx, means3D, means2D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp, viewmatrix,
+                bs: BatchSettings):
+        # an output the loss does not use arrives in backward as None instead of a zero tensor: a colour-only loss
+        # then gives the view matrices no gradient at all (and the kernels read no depth gradient: the same sums)
+        ctx.set_materialize_grads(False)
         dev = means3D.device
         if dev.type != "cuda":
             raise RuntimeError("pf3plat_b200 rasterizer needs CUDA tensors (there is no CPU fallback)")
@@ -217,8 +227,10 @@ class _RasterizeBatch(torch.autograd.Function):
             radii = torch.empty((V, P), dtype=torch.int32, device=dev)
             depth = torch.empty((V, H, W), dtype=torch.float32, device=dev) if bs.with_depth else None
             gout = GsOutputs(_ptr(color), _ptr(radii), _ptr(depth))
-            needs_grad = any(t is not None and t.requires_grad for t in
-                             (means3D, means2D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp))
+            want_view_z = bs.with_depth and viewmatrix.requires_grad
+            needs_grad = want_view_z or any(t is not None and t.requires_grad for t in
+                                            (means3D, means2D, shs, colors_precomp, opacities, scales, rotations,
+                                             cov3D_precomp))
             saved = ctypes.c_void_p()
             with _context_lock(dev, stream_ptr):
                 rc = _capi.lib().gs_forward(gctx, ctypes.byref(cfg), ctypes.byref(gin), ctypes.byref(gout),
@@ -237,6 +249,7 @@ class _RasterizeBatch(torch.autograd.Function):
             ctx.cfg_keep = keep
             ctx.dims = (S, P, V, M, H, W)
             ctx.want_means2D = means2D is not None and means2D.requires_grad
+            ctx.view_z = (viewmatrix.shape, viewmatrix.dtype) if want_view_z else None
         ctx.mark_non_differentiable(radii)
         if bs.with_depth:
             return color, radii, depth
@@ -270,25 +283,35 @@ class _RasterizeBatch(torch.autograd.Function):
                 "dL_dscales": e(S, P, 3) if ins["scales"] is not None else None,
                 "dL_drotations": e(S, P, 4) if ins["scales"] is not None else None,
                 "dL_dcov3D": e(S, P, 6) if ins["cov3D_precomp"] is not None else None,
+                "dL_dviewmatrix_z": e(V, 4) if ctx.view_z is not None and gdep is not None else None,
             }
             ig = GsInGrads(**{k: _ptr(t) for k, t in g.items()})
             with _context_lock(dev, stream_ptr):
                 rc = _capi.lib().gs_backward(gctx, ctypes.byref(cfg), ctypes.byref(gin), ctx.handle.ptr, ctypes.byref(og),
                                              ctypes.byref(ig), stream_ptr)
                 _capi.check(rc)
+            gview = None
+            if g["dL_dviewmatrix_z"] is not None:
+                # flat entries 2, 6, 10, 14 of the transposed matrix: its z column
+                gview = torch.zeros((V, 4, 4), dtype=torch.float32, device=dev)
+                gview[:, :, 2] = g["dL_dviewmatrix_z"]
+                shape, dtype = ctx.view_z
+                gview = gview.reshape(shape).to(dtype)
         return (g["dL_dmeans3D"], g["dL_dmeans2D"], g["dL_dshs"], g["dL_dcolors"], g["dL_dopacities"],
-                g["dL_dscales"], g["dL_drotations"], g["dL_dcov3D"], None)
+                g["dL_dscales"], g["dL_drotations"], g["dL_dcov3D"], gview, None)
 
 
 def rasterize_batch(bs: BatchSettings, means3D, opacities, shs=None, colors_precomp=None, scales=None,
                     rotations=None, cov3D_precomp=None, means2D=None):
     """Batched operator.  Shapes: means3D (S,P,3); opacities (S,P) or (S,P,1); shs (S,P,M,3); colors_precomp
     (V,P,3); scales (S,P,3); rotations (S,P,4); cov3D_precomp (S,P,6); means2D (V,P,3) (gradient sink only).
-    Returns (color (V,3,H,W), radii (V,P)[, depth (V,H,W)])."""
+    Returns (color (V,3,H,W), radii (V,P)[, depth (V,H,W)]).  With bs.with_depth, a bs.viewmatrix that requires grad
+    gets dL/ddepth's gradient in its z column (see _RasterizeBatch)."""
     _check_exclusive(shs, colors_precomp, scales, rotations, cov3D_precomp)
     # means2D exists in the reference op only as a sink for the screen-space gradient (cuda_splatting.py:93-97); the
     # batched entry neither allocates nor fills it unless the caller passes one
-    return _RasterizeBatch.apply(means3D, means2D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp, bs)
+    return _RasterizeBatch.apply(means3D, means2D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp,
+                                 bs.viewmatrix, bs)
 
 
 def _check_exclusive(shs, colors_precomp, scales, rotations, cov3D_precomp):
@@ -312,7 +335,8 @@ class GaussianRasterizer(nn.Module):
         f = lambda x: float(x)  # accepts python floats and 0-dim tensors (cuda_splatting.py:102-103 vs :195-196)
         return BatchSettings(
             image_height=int(rs.image_height), image_width=int(rs.image_width),
-            viewmatrix=rs.viewmatrix.reshape(1, 4, 4).to(device), projmatrix=rs.projmatrix.reshape(1, 4, 4),
+            # detached: the reference op gives viewmatrix no gradient, with or without return_depth
+            viewmatrix=rs.viewmatrix.detach().reshape(1, 4, 4).to(device), projmatrix=rs.projmatrix.reshape(1, 4, 4),
             campos=rs.campos.reshape(1, 3), bg=rs.bg.reshape(1, 3), sh_degree=int(rs.sh_degree),
             tanfovx=f(rs.tanfovx), tanfovy=f(rs.tanfovy), scale_modifier=float(rs.scale_modifier),
             prefiltered=bool(rs.prefiltered), with_depth=with_depth, debug=bool(rs.debug))
@@ -341,7 +365,7 @@ class GaussianRasterizer(nn.Module):
         u = lambda t: None if t is None else t.unsqueeze(0)
         bs = self._batch_settings(means3D.device, with_depth=return_depth)
         out = _RasterizeBatch.apply(u(means3D), u(means2D), u(shs), u(colors_precomp), u(opacities), u(scales),
-                                    u(rotations), u(cov3D_precomp), bs)
+                                    u(rotations), u(cov3D_precomp), bs.viewmatrix, bs)
         if return_depth:
             return out[0][0], out[1][0], out[2][0]
         return out[0][0], out[1][0]

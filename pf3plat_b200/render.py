@@ -79,17 +79,17 @@ def decoder_forward(means, covariances, harmonics, opacities, extrinsics, intrin
     (b,g,...), cameras (b,v,...).  Returns (color (b,v,3,h,w), depth (b,v,h,w) or None).  depth_mode "depth" is
     fused into the colour pass; the reference's other modes are served by `render_depth`.
 
-    Gradients: like the reference's colour pass, the fused pass gives the CAMERAS no gradient (the view matrices enter
-    the rasterizer detached on both sides, cuda_splatting.py:85-87 / make_view_batch) and routes dL/ddepth to the means
-    only.  The reference's depth pass, however, builds its fake colour z = (extrinsics^-1 @ mean).z in torch
-    (cuda_splatting.py:239-242), so its depth IS differentiable w.r.t. the extrinsics -- PF3plat trains with
-    depth_mode "depth" on predicted poses.  Whenever the extrinsics require grad, "depth" therefore takes the
-    reference's two-pass route (`render_depth`), which carries that gradient."""
+    Gradients: like the reference's colour pass, the colour gives the CAMERAS no gradient.  The reference's depth
+    pass builds its fake colour z = (extrinsics^-1 @ mean).z in torch (cuda_splatting.py:239-242), so its depth is
+    differentiable w.r.t. the extrinsics -- PF3plat trains with depth_mode "depth" on predicted poses.  The fused
+    channel gives exactly that gradient and no other: dL/ddepth reaches the z column of each view matrix
+    (make_view_batch carries it on to the extrinsics), besides the Gaussians.  A loss that does not read the depth
+    leaves the extrinsics without a gradient, as the reference does.  So "depth" is one render whether or not the
+    extrinsics require grad."""
     b, v = extrinsics.shape[:2]
     flat = lambda t: t.reshape(b * v, *t.shape[2:])
     bg = background_color.reshape(1, 3).expand(b * v, 3)
-    pose_grad = depth_mode == "depth" and extrinsics.requires_grad and torch.is_grad_enabled()
-    if (depth_mode is None or depth_mode == "depth") and not pose_grad:
+    if depth_mode is None or depth_mode == "depth":
         out = render_views(flat(extrinsics), flat(intrinsics), flat(near), flat(far), image_shape, bg, means,
                            covariances, harmonics, opacities, with_depth=depth_mode is not None)
         if depth_mode is None:
@@ -107,7 +107,9 @@ def decoder_forward(means, covariances, harmonics, opacities, extrinsics, intrin
 
 
 def render_depth(means, covariances, opacities, extrinsics, intrinsics, near, far, image_shape, mode: str = "depth"):
-    """`render_depth_cuda` (cuda_splatting.py:226-269) for (b,g,...) Gaussians and (b,v,...) cameras."""
+    """`render_depth_cuda` (cuda_splatting.py:226-269) for (b,g,...) Gaussians and (b,v,...) cameras: a second render
+    whose colour is the fake colour.  `decoder_forward` uses it for the modes other than "depth"; for "depth" it is the
+    reference's two-pass route, kept to compare the fused channel against."""
     b, v = extrinsics.shape[:2]
     flat = lambda t: t.reshape(b * v, *t.shape[2:])
     ext, nr, fr = flat(extrinsics), flat(near), flat(far)

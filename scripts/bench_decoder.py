@@ -3,20 +3,28 @@
   (1) the reference's call pattern: per-view GaussianRasterizer calls on v-fold repeated Gaussians + a second
       pass for depth (tests/ref_callsite.py restates cuda_splatting.py / decoder_splatting_cuda.py);
   (2) pf3plat_b200.render.decoder_forward: one batched call, depth fused.
-Prints one JSON line; both run OUR kernels -- this measures what the batched entry (SURVEY.md section 8(f).1) buys."""
+Prints one JSON line; both run OUR kernels -- this measures what the batched entry (SURVEY.md section 8(f).1) buys.
+
+GS_POSE=1 runs the leg PF3plat trains through instead (b defaults to 14): target extrinsics that require grad
+(predicted poses), loss = MSE on color[:, 1:-1] + a depth term.  It compares the two-pass route decoder_forward took for
+that case before the fused depth channel carried the camera gradient (render_views + render_depth) with
+decoder_forward, alternating, each on a stream (hence a rasterizer context and memory pool) of its own: forward,
+forward + backward, torch's peak allocation and the context pool's reservation, with the card's name and power limit."""
 import json
 import os
+import subprocess
 import sys
 import time
 
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-from pf3plat_b200.render import decoder_forward  # noqa: E402
+from pf3plat_b200.render import decoder_forward, render_depth, render_views  # noqa: E402
 from pf3plat_b200.synthetic import make_scene, make_target  # noqa: E402
 from tests.ref_callsite import render_depth_like_reference, render_like_reference  # noqa: E402
 
-b, v, P, hw = int(os.environ.get("GS_B", 2)), int(os.environ.get("GS_V", 3)), 131072, (256, 256)
+POSE = os.environ.get("GS_POSE") == "1"
+b, v, P, hw = int(os.environ.get("GS_B", 14 if POSE else 2)), int(os.environ.get("GS_V", 3)), 131072, (256, 256)
 steps = int(os.environ.get("GS_STEPS", 10))
 dev = torch.device("cuda:0")
 scs = [make_scene(P, v, *hw, seed=30 + k).to(dev) for k in range(b)]
@@ -65,6 +73,55 @@ def timeit(fn, grad):
         sys.stderr.write(f"{fn.__name__} grad={grad}: {per}\n")
     return 1e3 * (time.perf_counter() - t0) / steps
 
+
+def two_pass_route(grad):
+    e = ext.clone().requires_grad_(True)
+    L = [t.clone().requires_grad_(grad) for t in (means, cov, sh, opac)]
+    c = render_views(flat(e), flat(intr), flat(near), flat(far), hw, bg[None].expand(b * v, 3), *L).reshape(b, v, 3, *hw)
+    d = render_depth(L[0], L[1], L[3], e, intr, near, far, hw)
+    if grad:
+        (((c[:, 1:-1] - target[:, 1:-1]) ** 2).mean() + 1e-3 * d.mean()).backward()
+    return c
+
+
+def fused_route(grad):
+    e = ext.clone().requires_grad_(True)
+    L = [t.clone().requires_grad_(grad) for t in (means, cov, sh, opac)]
+    c, d = decoder_forward(*L, e, intr, near, far, hw, bg, depth_mode="depth")
+    if grad:
+        (((c[:, 1:-1] - target[:, 1:-1]) ** 2).mean() + 1e-3 * d.mean()).backward()
+    return c
+
+
+def pose_leg(rounds=3):
+    from pf3plat_b200.rasterizer import last_stats
+    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"],
+                       capture_output=True, text=True)
+    streams = {fn.__name__: torch.cuda.Stream(dev) for fn in (two_pass_route, fused_route)}
+    res = {k: {"fwd": [], "fwd_bwd": [], "peak_torch_mb": 0.0, "pool_reserved_mb": 0.0} for k in streams}
+    for _ in range(rounds):
+        for fn in (two_pass_route, fused_route):
+            name = fn.__name__
+            with torch.cuda.stream(streams[name]):
+                res[name]["fwd"].append(timeit(fn, False))
+                torch.cuda.reset_peak_memory_stats(dev)
+                res[name]["fwd_bwd"].append(timeit(fn, True))
+                res[name]["peak_torch_mb"] = max(res[name]["peak_torch_mb"], torch.cuda.max_memory_allocated(dev) / 2**20)
+                res[name]["pool_reserved_mb"] = max(res[name]["pool_reserved_mb"],
+                                                    last_stats(dev)["pool_reserved_bytes"] / 2**20)
+    out = {"config": f"GS_POSE: {b} scenes x {v} views, {P} Gaussians/scene, 256x256, extrinsics requiring grad, "
+                     f"loss MSE(color[:, 1:-1]) + 1e-3 mean(depth)", "steps": steps, "rounds (alternating)": rounds,
+           "device": torch.cuda.get_device_name(dev), "nvidia-smi name, power.limit": q.stdout.strip()}
+    for name, r in res.items():
+        out[name + "_ms"] = {k: {"median": sorted(r[k])[len(r[k]) // 2], "all": [round(x, 3) for x in r[k]]}
+                             for k in ("fwd", "fwd_bwd")}
+        out[name + "_memory_mb"] = {k: round(r[k], 1) for k in ("peak_torch_mb", "pool_reserved_mb")}
+    print(json.dumps(out))
+
+
+if POSE:
+    pose_leg()
+    sys.exit(0)
 
 out = {"config": f"{b} scenes x {v} views, {P} Gaussians/scene, 256x256, colour+depth", "steps": steps,
        "reference_call_pattern_ms": {"fwd": timeit(ref_fwd, False), "fwd_bwd": timeit(ref_fwd, True)},

@@ -34,7 +34,7 @@
 extern "C" {
 #endif
 
-#define GS_ABI_VERSION 2
+#define GS_ABI_VERSION 3
 
 #if defined(__GNUC__)
 #define GS_API __attribute__((visibility("default")))
@@ -53,7 +53,13 @@ enum {
 
 enum {
     GS_FLAG_DEPTH = 1u,        /* also composite camera-space z as a 4th channel (render_depth_cuda mode "depth", cuda_splatting.py:226-269, fused) */
-    GS_FLAG_PREFILTERED = 2u   /* GaussianRasterizationSettings.prefiltered */
+    GS_FLAG_PREFILTERED = 2u,  /* GaussianRasterizationSettings.prefiltered */
+    /* gs_backward: bit-reproducible gradients.  The composite backward adds its per-(view, Gaussian) terms as exact
+     * fixed-point integers (2^-80 resolution, terms up to 2^45 in magnitude; NaN, Inf or larger terms make that gradient
+     * component NaN) instead of float atomics, and the view-matrix gradient is summed in a fixed order.  Needs
+     * 244 B instead of 40 B of context scratch per (view, Gaussian); frames with ceil(H/4) * ceil(W/8) >= 2^21 and
+     * GS_TUNE_BWD_V1 are rejected (GS_ERR_INVALID).  The forward ignores it: it is deterministic already. */
+    GS_FLAG_DETERMINISTIC = 4u
 };
 
 enum {
@@ -253,7 +259,7 @@ typedef struct GsAdapterConfig {
     int32_t V;          /* cameras (leading batch dims of extrinsics, flattened) */
     int32_t R;          /* Gaussians per camera */
     int32_t d_sh;       /* SH coefficients per channel, (sh_degree + 1)^2 <= 25 */
-    int32_t reserved_;
+    uint32_t flags;     /* GS_ADAPTER_* */
     float scale_min;    /* GaussianAdapterCfg.gaussian_scale_min */
     float scale_max;    /* GaussianAdapterCfg.gaussian_scale_max */
     float eps;          /* forward(..., eps=1e-8) */
@@ -264,6 +270,12 @@ typedef struct GsAdapterConfig {
     const float *sh_rotation; /* device [V,d_sh,d_sh] or NULL */
     const float *sh_mask;     /* device [d_sh] (gaussian_adapter.py:39-46) */
 } GsAdapterConfig;
+
+enum {
+    /* gs_adapter_backward: bit-reproducible per-camera gradients (dL/dc2w, dL/dKinv, dL/dmultiplier).  Each CTA writes
+     * its partial sums to GsAdapterInGrads.scratch and a second kernel adds them in CTA order (no float atomics). */
+    GS_ADAPTER_DETERMINISTIC = 1u
+};
 
 typedef struct GsAdapterInputs {
     const float *coordinates;   /* device [V,R,2] */
@@ -290,11 +302,14 @@ typedef struct GsAdapterInGrads { /* any pointer may be NULL */
     float *c2w;           /* device [V,16]: through the means only (rotation is detached elsewhere, gaussian_adapter.py:81) */
     float *kinv;          /* device [V,9] */
     float *multiplier;    /* device [V] */
+    void *scratch;        /* device, gs_adapter_scratch_bytes(cfg) bytes, 16-byte aligned: required with
+                             GS_ADAPTER_DETERMINISTIC when c2w, kinv or multiplier is wanted; ignored otherwise */
 } GsAdapterInGrads;
 
 GS_API int gs_adapter_forward(const GsAdapterConfig *cfg, const GsAdapterInputs *in, const GsAdapterOutputs *out, void *stream);
 GS_API int gs_adapter_backward(const GsAdapterConfig *cfg, const GsAdapterInputs *in, const GsAdapterOutGrads *gout,
                         const GsAdapterInGrads *gin, void *stream);
+GS_API int64_t gs_adapter_scratch_bytes(const GsAdapterConfig *cfg); /* -1 for an invalid config */
 
 /*
  * Photometric training loss = PF3plat's LossMultiSSIM + LossMse (src/loss/loss_multissim.py:45-86, loss_mse.py:35),

@@ -12,10 +12,12 @@ from ctypes import POINTER, Structure, c_char_p, c_float, c_int, c_int32, c_int6
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "csrc", "libgsplat_b200.so")
-ABI_VERSION = 2
+ABI_VERSION = 3
 
 GS_FLAG_DEPTH = 1
 GS_FLAG_PREFILTERED = 2
+GS_FLAG_DETERMINISTIC = 4
+GS_ADAPTER_DETERMINISTIC = 1
 GS_TUNE_FORCE_RADIX_BINNING = 1
 GS_TUNE_NO_SPECULATION = 2
 GS_TUNE_SEPARATE_EMIT = 4
@@ -76,7 +78,7 @@ class GsStats(Structure):
 
 # every symbol include/gsplat_b200.h declares: name -> (restype, argtypes)
 class GsAdapterConfig(Structure):
-    _fields_ = [("V", c_int32), ("R", c_int32), ("d_sh", c_int32), ("reserved_", c_int32),
+    _fields_ = [("V", c_int32), ("R", c_int32), ("d_sh", c_int32), ("flags", c_uint32),
                 ("scale_min", c_float), ("scale_max", c_float), ("eps", c_float), ("reserved2_", c_float),
                 ("c2w", c_void_p), ("kinv", c_void_p), ("multiplier", c_void_p), ("sh_rotation", c_void_p),
                 ("sh_mask", c_void_p)]
@@ -98,7 +100,7 @@ class GsAdapterOutGrads(Structure):
 
 class GsAdapterInGrads(Structure):
     _fields_ = [("coordinates", c_void_p), ("depths", c_void_p), ("raw_gaussians", c_void_p), ("c2w", c_void_p),
-                ("kinv", c_void_p), ("multiplier", c_void_p)]
+                ("kinv", c_void_p), ("multiplier", c_void_p), ("scratch", c_void_p)]
 
 
 class GsLossConfig(Structure):
@@ -134,6 +136,7 @@ SYMBOLS = {
     "gs_adapter_forward": (c_int, [POINTER(GsAdapterConfig), POINTER(GsAdapterInputs), POINTER(GsAdapterOutputs), c_void_p]),
     "gs_adapter_backward": (c_int, [POINTER(GsAdapterConfig), POINTER(GsAdapterInputs), POINTER(GsAdapterOutGrads),
                                     POINTER(GsAdapterInGrads), c_void_p]),
+    "gs_adapter_scratch_bytes": (c_int64, [POINTER(GsAdapterConfig)]),
     "gs_photometric_scratch_bytes": (c_int64, [POINTER(GsLossConfig)]),
     "gs_photometric_forward": (c_int, [POINTER(GsLossConfig), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "gs_photometric_backward": (c_int, [POINTER(GsLossConfig), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,

@@ -92,11 +92,20 @@ class _AdapterFn(torch.autograd.Function):
         cfg = _capi.GsAdapterConfig(V=V, R=R, d_sh=d_sh, scale_min=scale_min, scale_max=scale_max, eps=eps,
                                     c2w=_ptr(keep[0]), kinv=_ptr(keep[1]), multiplier=_ptr(keep[2]),
                                     sh_rotation=_ptr(keep[3]), sh_mask=_ptr(keep[4]))
+        scratch = None
+        if torch.are_deterministic_algorithms_enabled():
+            # per-camera sums added in a fixed order instead of with float atomics: bit-reproducible dL/dc2w, dL/dKinv,
+            # dL/dmultiplier
+            cfg.flags = _capi.GS_ADAPTER_DETERMINISTIC
+            nbytes = _capi.lib().gs_adapter_scratch_bytes(ctypes.byref(cfg))
+            if nbytes < 0:
+                raise ValueError(f"invalid adapter configuration (V={V}, R={R}, d_sh={d_sh})")
+            scratch = torch.empty(max(nbytes, 1), dtype=torch.uint8, device=dev)
         inp = _capi.GsAdapterInputs(coordinates=_ptr(keep[5]), depths=_ptr(keep[6]), raw_gaussians=_ptr(keep[7]))
         gout = _capi.GsAdapterOutGrads(means=_ptr(gs[0]), covariances=_ptr(gs[1]), harmonics=_ptr(gs[2]),
                                        scales=_ptr(gs[3]), rotations=_ptr(gs[4]))
         gin = _capi.GsAdapterInGrads(coordinates=_ptr(d_coord), depths=_ptr(d_depth), raw_gaussians=_ptr(d_raw),
-                                     c2w=_ptr(d_c2w), kinv=_ptr(d_kinv), multiplier=_ptr(d_mult))
+                                     c2w=_ptr(d_c2w), kinv=_ptr(d_kinv), multiplier=_ptr(d_mult), scratch=_ptr(scratch))
         with torch.cuda.device(dev):
             stream = ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
             _capi.check(_capi.lib().gs_adapter_backward(ctypes.byref(cfg), ctypes.byref(inp), ctypes.byref(gout),

@@ -36,9 +36,11 @@ struct AdapterOutGrads {
 };
 struct AdapterInGrads {
     float *coords, *depths, *raw, *c2w, *kinv, *mult;
+    float *cam_partial;  // deterministic mode: [V][CTAs per camera][AD_CAM_SUMS] per-CTA sums (see k_adapter_bwd)
 };
 
 constexpr int AD_THREADS = 128;
+constexpr int AD_CAM_SUMS = 22;  // per-camera sums of the backward: dKinv 9 | dC 9 | dt 3 | dmultiplier 1
 constexpr int AD_MAX_DSH = 25;
 constexpr float AD_QUAT_EPS = 1e-8f;  // quaternion_to_matrix's own eps (PF3plat's src/model/encoder/common/gaussians.py:10)
 
@@ -220,6 +222,9 @@ __global__ void __launch_bounds__(AD_THREADS) k_adapter_fwd(const AdapterArgs a,
     }
 }
 
+// DET (GS_ADAPTER_DETERMINISTIC): the CTA's 22 per-camera sums are stored to gi_.cam_partial instead of being added to the
+// outputs with float atomics; k_adapter_cam_finalize adds them up in CTA order.
+template <bool DET>
 __global__ void __launch_bounds__(AD_THREADS)
 k_adapter_bwd(const AdapterArgs a, const AdapterOutGrads go, const AdapterInGrads gi_) {
     extern __shared__ __align__(128) unsigned char ad_smem[];
@@ -416,7 +421,12 @@ k_adapter_bwd(const AdapterArgs a, const AdapterOutGrads go, const AdapterInGrad
     const bool bulk_out = dst && ((reinterpret_cast<uintptr_t>(dst) & 15u) == 0) && ((out_bytes & 15u) == 0);
     if (bulk_out) fence_proxy_async_smem();
     __syncthreads();
-    if (tid < 22) {
+    if (DET && tid < AD_CAM_SUMS) {
+        float s = 0.f;
+#pragma unroll
+        for (int w = 0; w < AD_THREADS / 32; w++) s += h->red[w][tid];
+        gi_.cam_partial[((size_t)v * gridDim.x + blockIdx.x) * AD_CAM_SUMS + tid] = s;
+    } else if (tid < 22) {
         float s = 0.f;
 #pragma unroll
         for (int w = 0; w < AD_THREADS / 32; w++) s += h->red[w][tid];
@@ -441,6 +451,33 @@ k_adapter_bwd(const AdapterArgs a, const AdapterOutGrads go, const AdapterInGrad
             for (uint32_t k = tid; k < (uint32_t)n * a.C; k += AD_THREADS) dst[k] = draw_s[k];
         }
     }
+}
+
+// Deterministic mode: every element of dL/dKinv [V,9], dL/dc2w [V,16] (zeros outside the top 3x4 block) and
+// dL/dmultiplier [V] is the sum, in CTA order, of the CTAs' partials.
+__global__ void k_adapter_cam_finalize(int V, int ctas, const float *__restrict__ part, float *__restrict__ kinv,
+                                       float *__restrict__ c2w, float *__restrict__ mult) {
+    const int t = blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= V * 26) return;
+    const int v = t / 26, e = t - v * 26;  // e: 0-8 Kinv, 9-24 c2w (row-major), 25 multiplier
+    float *dst;
+    int src = -1;  // index of the partial, -1: a c2w entry the adapter gives no gradient
+    if (e < 9) {
+        dst = kinv ? kinv + (size_t)v * 9 + e : nullptr;
+        src = e;
+    } else if (e < 25) {
+        const int r = (e - 9) >> 2, col = (e - 9) & 3;
+        dst = c2w ? c2w + (size_t)v * 16 + (e - 9) : nullptr;
+        if (r < 3) src = col < 3 ? 9 + r * 3 + col : 18 + r;
+    } else {
+        dst = mult ? mult + v : nullptr;
+        src = 21;
+    }
+    if (!dst) return;
+    float s = 0.f;
+    if (src >= 0)
+        for (int k = 0; k < ctas; k++) s += part[((size_t)v * ctas + k) * AD_CAM_SUMS + src];
+    *dst = s;
 }
 
 constexpr size_t adapter_smem_bytes(int d_sh) { return AD_HDR_BYTES + (size_t)AD_THREADS * ((7 + 3 * d_sh) + 3 * d_sh) * 4; }
@@ -493,16 +530,38 @@ extern "C" GS_API int gs_adapter_backward(const GsAdapterConfig *cfg, const GsAd
     if (rc != GS_OK) return rc;
     if (!gout || !gin) return gs_set_error(GS_ERR_INVALID, "null adapter gradients");
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    if (gin->c2w && a.V) GS_CUDA_OK(cudaMemsetAsync(gin->c2w, 0, (size_t)a.V * 16 * 4, st));
-    if (gin->kinv && a.V) GS_CUDA_OK(cudaMemsetAsync(gin->kinv, 0, (size_t)a.V * 9 * 4, st));
-    if (gin->multiplier && a.V) GS_CUDA_OK(cudaMemsetAsync(gin->multiplier, 0, (size_t)a.V * 4, st));
+    const bool cam_grads = gin->c2w || gin->kinv || gin->multiplier;
+    const bool det = (cfg->flags & GS_ADAPTER_DETERMINISTIC) && cam_grads && (size_t)a.V * a.R > 0;
+    if (det && !gin->scratch)
+        return gs_set_error(GS_ERR_INVALID, "GS_ADAPTER_DETERMINISTIC needs gin->scratch (gs_adapter_scratch_bytes)");
+    if (!det) {  // the kernel accumulates into them (deterministic mode: k_adapter_cam_finalize writes every element)
+        if (gin->c2w && a.V) GS_CUDA_OK(cudaMemsetAsync(gin->c2w, 0, (size_t)a.V * 16 * 4, st));
+        if (gin->kinv && a.V) GS_CUDA_OK(cudaMemsetAsync(gin->kinv, 0, (size_t)a.V * 9 * 4, st));
+        if (gin->multiplier && a.V) GS_CUDA_OK(cudaMemsetAsync(gin->multiplier, 0, (size_t)a.V * 4, st));
+    }
     if ((size_t)a.V * a.R == 0) return GS_OK;
     const AdapterOutGrads go{gout->means, gout->covariances, gout->harmonics, gout->scales, gout->rotations};
-    const AdapterInGrads gi{gin->coordinates, gin->depths, gin->raw_gaussians, gin->c2w, gin->kinv, gin->multiplier};
+    const AdapterInGrads gi{gin->coordinates, gin->depths, gin->raw_gaussians, gin->c2w, gin->kinv, gin->multiplier,
+                            static_cast<float *>(gin->scratch)};
     const size_t smem = adapter_smem_bytes(a.d_sh);
-    GS_CUDA_OK(cudaFuncSetAttribute(k_adapter_bwd, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     dim3 grid((a.R + AD_THREADS - 1) / AD_THREADS, a.V);
-    k_adapter_bwd<<<grid, AD_THREADS, smem, st>>>(a, go, gi);
+    if (det) {
+        GS_CUDA_OK(cudaFuncSetAttribute(k_adapter_bwd<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        k_adapter_bwd<true><<<grid, AD_THREADS, smem, st>>>(a, go, gi);
+        GS_CUDA_OK(cudaGetLastError());
+        k_adapter_cam_finalize<<<(a.V * 26 + 127) / 128, 128, 0, st>>>(a.V, (int)grid.x, gi.cam_partial, gi.kinv, gi.c2w,
+                                                                       gi.mult);
+    } else {
+        GS_CUDA_OK(cudaFuncSetAttribute(k_adapter_bwd<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        k_adapter_bwd<false><<<grid, AD_THREADS, smem, st>>>(a, go, gi);
+    }
     GS_CUDA_OK(cudaGetLastError());
     return GS_OK;
+}
+
+extern "C" GS_API int64_t gs_adapter_scratch_bytes(const GsAdapterConfig *cfg) {
+    if (!cfg || cfg->V < 0 || cfg->R < 0 || cfg->V > 65535) return -1;
+    const int d = cfg->d_sh;
+    if (d != 1 && d != 4 && d != 9 && d != 16 && d != 25) return -1;
+    return (int64_t)cfg->V * ((cfg->R + AD_THREADS - 1) / AD_THREADS) * AD_CAM_SUMS * 4;
 }

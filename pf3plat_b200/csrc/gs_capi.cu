@@ -784,6 +784,15 @@ extern "C" int gs_backward(GsContext *ctx, const GsConfig *cfg, const GsInputs *
     c.flags = saved->flags;
     if (gin->dL_dviewmatrix_z && !(c.flags & GS_FLAG_DEPTH))
         return gs_set_error(GS_ERR_INVALID, "dL_dviewmatrix_z needs a forward with GS_FLAG_DEPTH");
+    const bool det = (cfg->flags & GS_FLAG_DETERMINISTIC) != 0;
+    if (det) {
+        if (cfg->tuning & GS_TUNE_BWD_V1)
+            return gs_set_error(GS_ERR_INVALID, "GS_FLAG_DETERMINISTIC: the round-1 backward kernel (GS_TUNE_BWD_V1) has no deterministic mode");
+        // every 8x4 pixel block of a view adds at most one term to an accumulator: the limbs' headroom bounds their number
+        if ((int64_t)((c.H + 3) / 4) * ((c.W + 7) / 8) >= GS_DET_MAX_TERMS)
+            return gs_set_error(GS_ERR_INVALID, "GS_FLAG_DETERMINISTIC: the frame has 2^21 or more 8x4 pixel blocks "
+                                                "(ceil(H/4) * ceil(W/8) must stay below 2097152)");
+    }
     const DevInputs di = make_dev_inputs(in);
     // the view-matrix gradient is written: zero it, then the kernels accumulate into it (nothing when there is no
     // incoming depth gradient: it stays zero and the default kernels run)
@@ -795,21 +804,34 @@ extern "C" int gs_backward(GsContext *ctx, const GsConfig *cfg, const GsInputs *
     const size_t n = (size_t)c.V * c.P;
     if (n == 0) return GS_OK;
 
-    rc = ctx->per_gaussian.reserve(n * GS_ACC_STRIDE * 4, 1.0, ctx->pool, st);
+    // Accumulators: n x GS_ACC_STRIDE floats; deterministic mode: n x GS_ACC_STRIDE x 3 int64 limbs + n poison masks
+    // (zeroed together), then the per-warp partials of the view-matrix gradient
+    const size_t acc_bytes = det ? n * (GS_ACC_STRIDE * GS_DET_LIMBS * 8 + 4) : n * GS_ACC_STRIDE * 4;
+    const size_t vz_off = align256(acc_bytes);
+    rc = ctx->per_gaussian.reserve(det ? vz_off + det_view_z_bytes(c) : acc_bytes, 1.0, ctx->pool, st);
     if (rc != GS_OK) return rc;
     float *acc = static_cast<float *>(ctx->per_gaussian.p);
+    DetAcc da{};
+    if (det) {
+        unsigned char *base = static_cast<unsigned char *>(ctx->per_gaussian.p);
+        da.acc = reinterpret_cast<unsigned long long *>(base);
+        da.poison = reinterpret_cast<uint32_t *>(base + n * GS_ACC_STRIDE * GS_DET_LIMBS * 8);
+        da.view_z = reinterpret_cast<float *>(base + vz_off);
+        acc = nullptr;
+    }
     {
         StageTimer t(ctx, GS_STAGE_COMPOSITE_BWD, st);
-        GS_CUDA_OK(cudaMemsetAsync(acc, 0, n * GS_ACC_STRIDE * 4, st));
-        rc = launch_composite_bwd(c, *saved, gout->dL_dcolor, gout->dL_ddepth, acc, st, (cfg->tuning & GS_TUNE_BWD_V1) ? 1 : ((cfg->tuning & GS_TUNE_BWD_OCC4) ? 2 : 0));
+        GS_CUDA_OK(cudaMemsetAsync(ctx->per_gaussian.p, 0, acc_bytes, st));
+        rc = launch_composite_bwd(c, *saved, gout->dL_dcolor, gout->dL_ddepth, acc, st, (cfg->tuning & GS_TUNE_BWD_V1) ? 1 : ((cfg->tuning & GS_TUNE_BWD_OCC4) ? 2 : 0), da);
         if (rc != GS_OK) return rc;
     }
     {
         StageTimer t(ctx, GS_STAGE_PREPROCESS_BWD, st);
-        rc = launch_preprocess_bwd(c, di, *saved, acc, g, st, (cfg->tuning & GS_TUNE_PBWD_2PHASE) ? 1 : 0);
+        rc = launch_preprocess_bwd(c, di, *saved, acc, g, st, (cfg->tuning & GS_TUNE_PBWD_2PHASE) ? 1 : 0, da);
         if (rc != GS_OK) return rc;
     }
     ctx->stats.kernel_launches += 2;  // k_composite_bwd, k_preprocess_bwd
+    if (det && g.dL_dviewmatrix_z) ctx->stats.kernel_launches += 1;  // k_view_z_finalize
     return GS_OK;
 }
 

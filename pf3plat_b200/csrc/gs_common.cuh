@@ -14,6 +14,7 @@
 #include <stdint.h>
 
 #include "../../include/gsplat_b200.h"
+#include "gs_det.cuh"
 
 #define GS_TILE 16
 #define GS_TILE_PX (GS_TILE * GS_TILE)
@@ -113,13 +114,26 @@ int bin_sort_fallback(const DevCfg &c, int64_t D, const float4 *rec0, const floa
                       const ushort4 *rects, void *scratch, size_t scratch_bytes, uint32_t *point_list, uint2 *ranges,
                       cudaStream_t st);
 
+// Deterministic backward (GS_FLAG_DETERMINISTIC, DESIGN.md 5.11): the composite backward adds its terms into exact
+// fixed-point accumulators (gs_det.cuh) instead of the float ones, and the view-matrix gradient is summed in a fixed
+// order from per-warp partials.  All NULL on the default path.
+struct DetAcc {
+    unsigned long long *acc;  // [V*P][GS_ACC_STRIDE][GS_DET_LIMBS], zeroed
+    uint32_t *poison;         // [V*P], zeroed: bit k = component k received a non-finite or out-of-range term
+    float *view_z;            // [V][warps of one scene's preprocess-backward grid][4] (needs no zeroing)
+};
+
 int launch_composite_fwd(const DevCfg &c, const GsSaved &s, float *color, float *depth, cudaStream_t st,
                          int variant = 0 /* 2: the persistent warp-specialised kernel (GS_TUNE_FWD_WS) */);
 int launch_composite_bwd(const DevCfg &c, const GsSaved &s, const float *dL_dcolor, const float *dL_ddepth,
                          float *grad_acc /* [V*P*GS_ACC_STRIDE], zeroed */, cudaStream_t st,
-                         int variant = 0 /* 1: the round-1 kernel (GS_TUNE_BWD_V1) */);
+                         int variant = 0 /* 1: the round-1 kernel (GS_TUNE_BWD_V1) */,
+                         const DetAcc &det = DetAcc{} /* det.acc != NULL: fixed-point accumulators instead of grad_acc */);
 int launch_preprocess_bwd(const DevCfg &c, const DevInputs &in, const GsSaved &s, const float *grad_acc,
-                          const GsInGrads &g, cudaStream_t st, int variant = 0 /* 1: the two-phase kernel (GS_TUNE_PBWD_2PHASE) */);
+                          const GsInGrads &g, cudaStream_t st, int variant = 0 /* 1: the two-phase kernel (GS_TUNE_PBWD_2PHASE) */,
+                          const DetAcc &det = DetAcc{});
+// bytes of DetAcc::view_z for a configuration
+size_t det_view_z_bytes(const DevCfg &c);
 
 // per (view,Gaussian) accumulator written by the composite backward:
 //   0-2 dL/drgb, 3-4 dL/dmean2D (NDC-scaled), 5-7 dL/dconic (a, b stored once, c), 8 dL/dopacity, 9 dL/dz

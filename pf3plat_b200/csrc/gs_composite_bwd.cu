@@ -281,13 +281,19 @@ struct Cb2Smem {
     uint32_t max[CB_THREADS / 32];
 };
 
-template <bool DEPTH, int CB_BATCH, int MINB>
+// DET (GS_FLAG_DETERMINISTIC): the ten sums of a (warp, Gaussian) -- already independent of scheduling, they depend only
+// on the order of the tile list -- are added into exact fixed-point accumulators (gs_det.cuh) with 64-bit integer REDs
+// instead of float REDs, so the totals do not depend on the order in which warps arrive.  A term with no encoding
+// (non-finite, out of range) sets its component's bit in the poison mask.  DET = false is the default kernel,
+// instruction for instruction (the two trailing parameters are unused).
+template <bool DEPTH, int CB_BATCH, int MINB, bool DET = false>
 __global__ void __launch_bounds__(CB_THREADS, MINB)
 k_composite_bwd(const DevCfg c, const float4 *__restrict__ rec0, const float4 *__restrict__ rec1,
                 const float4 *__restrict__ rec2, const uint32_t *__restrict__ point_list,
                 const uint2 *__restrict__ ranges, const float *__restrict__ final_T,
                 const uint32_t *__restrict__ n_contrib, const float *__restrict__ dL_dcolor,
-                const float *__restrict__ dL_ddepth, float *__restrict__ acc) {
+                const float *__restrict__ dL_ddepth, float *__restrict__ acc,
+                unsigned long long *__restrict__ det_acc, uint32_t *__restrict__ det_poison) {
     extern __shared__ __align__(16) unsigned char cb_smem[];
     Cb2Smem<CB_BATCH> &sm = *reinterpret_cast<Cb2Smem<CB_BATCH> *>(cb_smem);
     auto &s_rec = sm.rec;
@@ -391,13 +397,33 @@ k_composite_bwd(const DevCfg c, const float4 *__restrict__ rec0, const float4 *_
         if (DEPTH) cz += __shfl_xor_sync(0xffffffffu, cz, 16);
         if (rs < nslots) {
             // lanes of half 0 retire components 0-4, lanes of half 1 components 5-9: five RED instructions, 32 addresses each
-            float *dst = acc + (rbase + __float_as_uint(gb.z)) * GS_ACC_STRIDE + 5 * rh;
-            const float v0 = rh ? g5 : c0, v1 = rh ? g6 : c1, v2 = rh ? g7 : c2, v3 = rh ? M0 : g3, v4 = rh ? cz : g4;
-            if (v0 != 0.f) atomicAdd(dst + 0, v0);
-            if (v1 != 0.f) atomicAdd(dst + 1, v1);
-            if (v2 != 0.f) atomicAdd(dst + 2, v2);
-            if (v3 != 0.f) atomicAdd(dst + 3, v3);
-            if (v4 != 0.f) atomicAdd(dst + 4, v4);
+            if constexpr (DET) {
+                const size_t e = rbase + __float_as_uint(gb.z);
+                unsigned long long *dst = det_acc + (e * GS_ACC_STRIDE + 5 * rh) * GS_DET_LIMBS;
+                const float vals[5] = {rh ? g5 : c0, rh ? g6 : c1, rh ? g7 : c2, rh ? M0 : g3, rh ? cz : g4};
+                uint32_t bad = 0;
+#pragma unroll
+                for (int q = 0; q < 5; q++) {
+                    if (vals[q] == 0.f) continue;
+                    long long limb[GS_DET_LIMBS];
+                    if (!gs_det_encode(vals[q], limb)) {
+                        bad |= 1u << (5 * rh + q);
+                        continue;
+                    }
+#pragma unroll
+                    for (int k = 0; k < GS_DET_LIMBS; k++)  // at most two of the three are non-zero
+                        if (limb[k]) atomicAdd(dst + q * GS_DET_LIMBS + k, (unsigned long long)limb[k]);
+                }
+                if (bad) atomicOr(det_poison + e, bad);
+            } else {
+                float *dst = acc + (rbase + __float_as_uint(gb.z)) * GS_ACC_STRIDE + 5 * rh;
+                const float v0 = rh ? g5 : c0, v1 = rh ? g6 : c1, v2 = rh ? g7 : c2, v3 = rh ? M0 : g3, v4 = rh ? cz : g4;
+                if (v0 != 0.f) atomicAdd(dst + 0, v0);
+                if (v1 != 0.f) atomicAdd(dst + 1, v1);
+                if (v2 != 0.f) atomicAdd(dst + 2, v2);
+                if (v3 != 0.f) atomicAdd(dst + 3, v3);
+                if (v4 != 0.f) atomicAdd(dst + 4, v4);
+            }
         }
         __syncwarp();  // the rows may be overwritten
     };
@@ -488,7 +514,7 @@ k_composite_bwd(const DevCfg c, const float4 *__restrict__ rec0, const float4 *_
 }  // namespace
 
 int launch_composite_bwd(const DevCfg &c, const GsSaved &s, const float *dL_dcolor, const float *dL_ddepth,
-                         float *grad_acc, cudaStream_t st, int variant) {
+                         float *grad_acc, cudaStream_t st, int variant, const DetAcc &det) {
     if (c.V == 0 || c.ntiles == 0) return GS_OK;
     dim3 grid(c.ntiles, c.V);
     if (variant != 1) {
@@ -498,12 +524,17 @@ int launch_composite_bwd(const DevCfg &c, const GsSaved &s, const float *dL_dcol
         auto launch = [&](auto kern, size_t smem) -> int {
             GS_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
             kern<<<grid, CB_THREADS, smem, st>>>(c, s.rec0, s.rec1, s.rec2, s.point_list, s.ranges, s.final_T, s.n_contrib,
-                                                 dL_dcolor, dL_ddepth, grad_acc);
+                                                 dL_dcolor, dL_ddepth, grad_acc, det.acc, det.poison);
             return GS_OK;
         };
         const bool dep = (c.flags & GS_FLAG_DEPTH) != 0;
         int rc;
-        if (variant == 2)
+        if (det.acc) {
+            if (variant == 2)
+                rc = dep ? launch(k_composite_bwd<true, 128, 4, true>, sizeof(Cb2Smem<128>)) : launch(k_composite_bwd<false, 128, 4, true>, sizeof(Cb2Smem<128>));
+            else
+                rc = dep ? launch(k_composite_bwd<true, 256, 3, true>, sizeof(Cb2Smem<256>)) : launch(k_composite_bwd<false, 256, 3, true>, sizeof(Cb2Smem<256>));
+        } else if (variant == 2)
             rc = dep ? launch(k_composite_bwd<true, 128, 4>, sizeof(Cb2Smem<128>)) : launch(k_composite_bwd<false, 128, 4>, sizeof(Cb2Smem<128>));
         else
             rc = dep ? launch(k_composite_bwd<true, 256, 3>, sizeof(Cb2Smem<256>)) : launch(k_composite_bwd<false, 256, 3>, sizeof(Cb2Smem<256>));
@@ -511,6 +542,7 @@ int launch_composite_bwd(const DevCfg &c, const GsSaved &s, const float *dL_dcol
         GS_CUDA_OK(cudaGetLastError());
         return GS_OK;
     }
+    if (det.acc) return gs_set_error(GS_ERR_INVALID, "the round-1 backward kernel has no deterministic mode");
     // Batch of 256 entries, registers unbounded (80 -> 3 CTAs/SM).  On C2 a batch of 128 with registers bounded
     // to 64 (4 CTAs/SM, 32 B of spills) and a batch of 128 at 3 CTAs/SM were both slower -- the kernel is issue-bound, more resident warps do not help it.
     constexpr int BATCH = CB_BATCH_MAX, MINB = 3;

@@ -96,13 +96,46 @@ __device__ __forceinline__ void red_view_z_grad(float *dst, float a, float b, fl
     }
 }
 
+// Deterministic mode: the warp's sum goes to its own slot of det.view_z ([V][warps of the scene's grid][4]) with a
+// plain store, and k_view_z_finalize adds the slots up in warp order.  Same calling rules as red_view_z_grad.
+template <bool DET>
+__device__ __forceinline__ void view_z_grad(const GsInGrads &g, const DetAcc &det, int v, float a, float b, float c,
+                                            float d) {
+    if constexpr (DET) {
+#pragma unroll
+        for (int off = 16; off > 0; off >>= 1) {
+            a += __shfl_xor_sync(0xffffffffu, a, off);
+            b += __shfl_xor_sync(0xffffffffu, b, off);
+            c += __shfl_xor_sync(0xffffffffu, c, off);
+            d += __shfl_xor_sync(0xffffffffu, d, off);
+        }
+        if ((threadIdx.x & 31) == 0) {
+            const size_t warps = (size_t)gridDim.x * (PB_THREADS / 32);
+            const size_t w = (size_t)blockIdx.x * (PB_THREADS / 32) + (threadIdx.x >> 5);
+            reinterpret_cast<float4 *>(det.view_z)[(size_t)v * warps + w] = make_float4(a, b, c, d);
+        }
+    } else {
+        red_view_z_grad(g.dL_dviewmatrix_z + (size_t)v * 4, a, b, c, d);
+    }
+}
+
+// The decoded fixed-point accumulators of (view, Gaussian) o (deterministic mode), written to out; returns out.
+__device__ __forceinline__ const float *load_det_acc(const DetAcc &det, size_t o, float out[GS_ACC_STRIDE]) {
+    const uint32_t bad = det.poison[o];
+    const long long *l = reinterpret_cast<const long long *>(det.acc) + o * GS_ACC_STRIDE * GS_DET_LIMBS;
+#pragma unroll
+    for (int k = 0; k < GS_ACC_STRIDE; k++) out[k] = gs_det_decode(l + k * GS_DET_LIMBS, (bad >> k) & 1u);
+    return out;
+}
+
 // VIEW_Z: also write g.dL_dviewmatrix_z, the depth channel's gradient w.r.t. the z column of each view matrix
 // (z = view[2] m.x + view[6] m.y + view[10] m.z + view[14], m the view-scaled mean).  The default instantiations
-// (VIEW_Z = false) are the kernels without it, instruction for instruction.
-template <bool HAS_SH, int MINB, bool VIEW_Z = false>
+// (VIEW_Z = false) are the kernels without it, instruction for instruction.  DET: the accumulators are the fixed-point
+// ones of the deterministic backward (det.acc, det.poison) and the view-matrix gradient goes through det.view_z.
+template <bool HAS_SH, int MINB, bool VIEW_Z = false, bool DET = false>
 __global__ void __launch_bounds__(PB_THREADS, MINB)
 k_preprocess_bwd(const DevCfg c, const DevInputs in, const uint8_t *__restrict__ meta, const float *__restrict__ acc,
-                    const GsInGrads g) {
+                    const GsInGrads g, const DetAcc det) {
     extern __shared__ __align__(128) unsigned char smem_raw[];
     PbSmem *sm = reinterpret_cast<PbSmem *>(smem_raw);
     float *sh_s = reinterpret_cast<float *>(smem_raw + PB_SMEM_HDR);
@@ -168,16 +201,18 @@ k_preprocess_bwd(const DevCfg c, const DevInputs in, const uint8_t *__restrict__
             __syncthreads();
         }
         if (!active) {
-            if (VIEW_Z) red_view_z_grad(g.dL_dviewmatrix_z + (size_t)v * 4, 0.f, 0.f, 0.f, 0.f);
+            if (VIEW_Z) view_z_grad<DET>(g, det, v, 0.f, 0.f, 0.f, 0.f);
             continue;
         }
         const ViewCam &cam = sm->cams[vi % GS_CAM_CHUNK];
         const size_t o = (size_t)v * c.P + i;
         const uint32_t mb = meta[o];
         float m2d[2] = {0.f, 0.f}, gcol[3] = {0.f, 0.f, 0.f};
-        if (VIEW_Z && !(mb & GS_META_VISIBLE)) red_view_z_grad(g.dL_dviewmatrix_z + (size_t)v * 4, 0.f, 0.f, 0.f, 0.f);
+        if (VIEW_Z && !(mb & GS_META_VISIBLE)) view_z_grad<DET>(g, det, v, 0.f, 0.f, 0.f, 0.f);
         if (mb & GS_META_VISIBLE) {
             const float *a = acc + o * GS_ACC_STRIDE;
+            float a_det[GS_ACC_STRIDE];
+            if constexpr (DET) a = load_det_acc(det, o, a_det);
             gcol[0] = a[0]; gcol[1] = a[1]; gcol[2] = a[2];
             m2d[0] = a[3]; m2d[1] = a[4];
             const float gcx = a[5], gcy = a[6], gcz = a[7];
@@ -248,7 +283,7 @@ k_preprocess_bwd(const DevCfg c, const DevInputs in, const uint8_t *__restrict__
             gm[0] += cam.view[2] * gz;
             gm[1] += cam.view[6] * gz;
             gm[2] += cam.view[10] * gz;
-            if (VIEW_Z) red_view_z_grad(g.dL_dviewmatrix_z + (size_t)v * 4, gz * m.x, gz * m.y, gz * m.z, gz);
+            if (VIEW_Z) view_z_grad<DET>(g, det, v, gz * m.x, gz * m.y, gz * m.z, gz);
             // ---- colour -> SH coefficients and mean (view direction) ----
             if (HAS_SH) {
                 const float d[3] = {m.x - cam.campos[0], m.y - cam.campos[1], m.z - cam.campos[2]};
@@ -372,10 +407,10 @@ k_preprocess_bwd(const DevCfg c, const DevInputs in, const uint8_t *__restrict__
 // camera / direction / basis work is redone per phase), and slower.  The single-pass kernel stays the default.
 constexpr int PB2_MIN_CTAS = 6;
 
-template <bool HAS_SH, bool VIEW_Z = false>
+template <bool HAS_SH, bool VIEW_Z = false, bool DET = false>
 __global__ void __launch_bounds__(PB_THREADS, PB2_MIN_CTAS)
 k_preprocess_bwd_2phase(const DevCfg c, const DevInputs in, const uint8_t *__restrict__ meta, const float *__restrict__ acc,
-                 const GsInGrads g) {
+                 const GsInGrads g, const DetAcc det) {
     extern __shared__ __align__(128) unsigned char smem_raw[];
     PbSmem *sm = reinterpret_cast<PbSmem *>(smem_raw);
     float *sh_s = reinterpret_cast<float *>(smem_raw + PB_SMEM_HDR);
@@ -450,16 +485,18 @@ k_preprocess_bwd_2phase(const DevCfg c, const DevInputs in, const uint8_t *__res
                 __syncthreads();
             }
             if (!active) {
-                if (VIEW_Z) red_view_z_grad(g.dL_dviewmatrix_z + (size_t)v * 4, 0.f, 0.f, 0.f, 0.f);
+                if (VIEW_Z) view_z_grad<DET>(g, det, v, 0.f, 0.f, 0.f, 0.f);
                 continue;
             }
             const ViewCam &cam = sm->cams[vi % GS_CAM_CHUNK];
             const size_t o = (size_t)v * c.P + i;
             const uint32_t mb = meta[o];
             float m2d[2] = {0.f, 0.f}, gcol[3] = {0.f, 0.f, 0.f};
-            if (VIEW_Z && !(mb & GS_META_VISIBLE)) red_view_z_grad(g.dL_dviewmatrix_z + (size_t)v * 4, 0.f, 0.f, 0.f, 0.f);
+            if (VIEW_Z && !(mb & GS_META_VISIBLE)) view_z_grad<DET>(g, det, v, 0.f, 0.f, 0.f, 0.f);
             if (mb & GS_META_VISIBLE) {
                 const float *a = acc + o * GS_ACC_STRIDE;
+                float a_det[GS_ACC_STRIDE];
+                if constexpr (DET) a = load_det_acc(det, o, a_det);
                 gcol[0] = a[0]; gcol[1] = a[1]; gcol[2] = a[2];
                 m2d[0] = a[3]; m2d[1] = a[4];
                 const float gcx = a[5], gcy = a[6], gcz = a[7];
@@ -530,7 +567,7 @@ k_preprocess_bwd_2phase(const DevCfg c, const DevInputs in, const uint8_t *__res
                 gm[0] += cam.view[2] * gz;
                 gm[1] += cam.view[6] * gz;
                 gm[2] += cam.view[10] * gz;
-                if (VIEW_Z) red_view_z_grad(g.dL_dviewmatrix_z + (size_t)v * 4, gz * m.x, gz * m.y, gz * m.z, gz);
+                if (VIEW_Z) view_z_grad<DET>(g, det, v, gz * m.x, gz * m.y, gz * m.z, gz);
 #pragma unroll
                 for (int k = 0; k < 3; k++) gmean[k] += s * gm[k];
             }
@@ -607,7 +644,12 @@ k_preprocess_bwd_2phase(const DevCfg c, const DevInputs in, const uint8_t *__res
                 const size_t o = (size_t)v * c.P + i;
                 const uint32_t mb = meta[o];
                 if (!(mb & GS_META_VISIBLE) || (mb & (1u << ch))) continue;   // invisible, or this channel was clamped at 0
-                const float gch = acc[o * GS_ACC_STRIDE + ch];
+                float gch;
+                if constexpr (DET)
+                    gch = gs_det_decode(reinterpret_cast<const long long *>(det.acc) + (o * GS_ACC_STRIDE + ch) * GS_DET_LIMBS,
+                                        (det.poison[o] >> ch) & 1u);
+                else
+                    gch = acc[o * GS_ACC_STRIDE + ch];
                 const float s = cam.scale;
                 const float d[3] = {mean.x * s - cam.campos[0], mean.y * s - cam.campos[1], mean.z * s - cam.campos[2]};
                 const float len2 = d[0] * d[0] + d[1] * d[1] + d[2] * d[2];
@@ -654,35 +696,58 @@ k_preprocess_bwd_2phase(const DevCfg c, const DevInputs in, const uint8_t *__res
     }
 }
 
-template <bool VIEW_Z>
+template <bool VIEW_Z, bool DET>
 int launch_preprocess_bwd_t(const DevCfg &c, const DevInputs &in, const GsSaved &s, const float *grad_acc,
-                            const GsInGrads &g, cudaStream_t st, int variant) {
+                            const GsInGrads &g, cudaStream_t st, int variant, const DetAcc &det) {
     dim3 grid((c.P + PB_THREADS - 1) / PB_THREADS, c.S);
     if (variant != 1) {  // single pass over the views (default)
         if (in.shs) {
             size_t smem = PB_SMEM_HDR + (size_t)PB_THREADS * c.M * 12;
-            GS_CUDA_OK(cudaFuncSetAttribute(k_preprocess_bwd<true, PB_MIN_CTAS, VIEW_Z>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-            k_preprocess_bwd<true, PB_MIN_CTAS, VIEW_Z><<<grid, PB_THREADS, smem, st>>>(c, in, s.meta, grad_acc, g);
+            GS_CUDA_OK(cudaFuncSetAttribute(k_preprocess_bwd<true, PB_MIN_CTAS, VIEW_Z, DET>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            k_preprocess_bwd<true, PB_MIN_CTAS, VIEW_Z, DET><<<grid, PB_THREADS, smem, st>>>(c, in, s.meta, grad_acc, g, det);
         } else {
-            k_preprocess_bwd<false, PB_MIN_CTAS, VIEW_Z><<<grid, PB_THREADS, PB_SMEM_HDR, st>>>(c, in, s.meta, grad_acc, g);
+            k_preprocess_bwd<false, PB_MIN_CTAS, VIEW_Z, DET><<<grid, PB_THREADS, PB_SMEM_HDR, st>>>(c, in, s.meta, grad_acc, g, det);
         }
     } else if (in.shs) {
         size_t smem = PB_SMEM_HDR + (size_t)PB_THREADS * (c.M <= PB_SH_EVAL ? c.M * 3 : PB_SH_EVAL * 3 + 1) * 4;
-        GS_CUDA_OK(cudaFuncSetAttribute(k_preprocess_bwd_2phase<true, VIEW_Z>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        k_preprocess_bwd_2phase<true, VIEW_Z><<<grid, PB_THREADS, smem, st>>>(c, in, s.meta, grad_acc, g);
+        GS_CUDA_OK(cudaFuncSetAttribute(k_preprocess_bwd_2phase<true, VIEW_Z, DET>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        k_preprocess_bwd_2phase<true, VIEW_Z, DET><<<grid, PB_THREADS, smem, st>>>(c, in, s.meta, grad_acc, g, det);
     } else {
-        k_preprocess_bwd_2phase<false, VIEW_Z><<<grid, PB_THREADS, PB_SMEM_HDR, st>>>(c, in, s.meta, grad_acc, g);
+        k_preprocess_bwd_2phase<false, VIEW_Z, DET><<<grid, PB_THREADS, PB_SMEM_HDR, st>>>(c, in, s.meta, grad_acc, g, det);
     }
     GS_CUDA_OK(cudaGetLastError());
     return GS_OK;
 }
 
+// dL/dviewmatrix_z[v][k] = sum over w, in order, of the per-warp partials view_z[v][w][k]
+__global__ void k_view_z_finalize(int V, int warps, const float *__restrict__ view_z, float *__restrict__ out) {
+    const int t = blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= V * 4) return;
+    const int v = t >> 2, k = t & 3;
+    const float *p = view_z + (size_t)v * warps * 4 + k;
+    float sum = 0.f;
+    for (int w = 0; w < warps; w++) sum += p[(size_t)w * 4];
+    out[t] = sum;
+}
+
+int view_z_warps(const DevCfg &c) { return (c.P + PB_THREADS - 1) / PB_THREADS * (PB_THREADS / 32); }
+
 }  // namespace
 
-// g.dL_dviewmatrix_z non-NULL selects the VIEW_Z kernels; the caller has zeroed it (the kernels accumulate into it).
+size_t det_view_z_bytes(const DevCfg &c) { return (size_t)c.V * view_z_warps(c) * 4 * sizeof(float); }
+
+// g.dL_dviewmatrix_z non-NULL selects the VIEW_Z kernels; the caller has zeroed it (the kernels accumulate into it, or in
+// deterministic mode k_view_z_finalize writes it).  det.acc non-NULL selects the deterministic kernels.
 int launch_preprocess_bwd(const DevCfg &c, const DevInputs &in, const GsSaved &s, const float *grad_acc,
-                          const GsInGrads &g, cudaStream_t st, int variant) {
+                          const GsInGrads &g, cudaStream_t st, int variant, const DetAcc &det) {
     if (c.P == 0) return GS_OK;
-    return g.dL_dviewmatrix_z ? launch_preprocess_bwd_t<true>(c, in, s, grad_acc, g, st, variant)
-                              : launch_preprocess_bwd_t<false>(c, in, s, grad_acc, g, st, variant);
+    if (!det.acc)
+        return g.dL_dviewmatrix_z ? launch_preprocess_bwd_t<true, false>(c, in, s, grad_acc, g, st, variant, det)
+                                  : launch_preprocess_bwd_t<false, false>(c, in, s, grad_acc, g, st, variant, det);
+    if (!g.dL_dviewmatrix_z) return launch_preprocess_bwd_t<false, true>(c, in, s, grad_acc, g, st, variant, det);
+    const int rc = launch_preprocess_bwd_t<true, true>(c, in, s, grad_acc, g, st, variant, det);
+    if (rc != GS_OK) return rc;
+    k_view_z_finalize<<<(c.V * 4 + 127) / 128, 128, 0, st>>>(c.V, view_z_warps(c), det.view_z, g.dL_dviewmatrix_z);
+    GS_CUDA_OK(cudaGetLastError());
+    return GS_OK;
 }

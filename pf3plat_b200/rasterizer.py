@@ -197,7 +197,7 @@ class _RasterizeBatch(torch.autograd.Function):
     one only through the fused depth channel (bs.with_depth), as the reference's depth pass gives its cameras one
     through its fake colour z (cuda_splatting.py:239-242): dL/dviewmatrix is zero outside the z column, and None when
     the depth is not part of the loss.  Colour, projection and culling give the cameras no gradient, as in the
-    reference op."""
+    reference op.  Under torch.use_deterministic_algorithms(True) the backward is bit-reproducible."""
 
     @staticmethod
     def forward(ctx, means3D, means2D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp, viewmatrix,
@@ -270,6 +270,9 @@ class _RasterizeBatch(torch.autograd.Function):
             stream_ptr = torch.cuda.current_stream(dev).cuda_stream
             gctx = _context(dev, stream_ptr)
             cfg = _make_config(bs, S, P, M, keep)
+            if torch.are_deterministic_algorithms_enabled():
+                # bit-reproducible gradients: fixed-point accumulation instead of float atomics (DESIGN.md 5.11)
+                cfg.flags |= _capi.GS_FLAG_DETERMINISTIC
             gin = GsInputs(**{k: _ptr(t) for k, t in ins.items()})
             gcol = _f32c(grad_color) if grad_color is not None else torch.zeros((V, 3, H, W), device=dev)
             gdep = _f32c(grad_depth) if (bs.with_depth and grad_depth is not None) else None

@@ -19,6 +19,25 @@ namespace {
 constexpr int PRE_THREADS = 128;
 constexpr int EMIT_BATCH = 4;  // cursor atomics in flight per thread
 
+// Knock-out builds for scripts/preprocess_ablation.py (-DGS_PRE_ABLATE=<mask>; 0, the product build, removes nothing).
+// Each bit drops one piece of k_preprocess's work on the speculative path; what the compiler could dead-code around it is
+// kept alive by abl_sink.  The results of such a build are wrong by design: it exists to be timed.
+#ifndef GS_PRE_ABLATE
+#define GS_PRE_ABLATE 0
+#endif
+constexpr unsigned ABL = GS_PRE_ABLATE;
+constexpr unsigned ABL_EMIT = 1;    // fused emission: no cursor atomics, no bucket stores (the tile tests stay)
+constexpr unsigned ABL_TESTS = 2;   // the candidate tile tests (every candidate of the 3-sigma square passes)
+constexpr unsigned ABL_SH = 4;      // SH staging and eval_sh: the colour is a constant
+constexpr unsigned ABL_REC = 8;     // the rec0..rec2 stores
+constexpr unsigned ABL_RRM = 16;    // the radii / rects / meta stores
+constexpr unsigned ABL_BAR = 32;    // the barrier pair of the first camera chunk (its cameras ride on the SH barrier)
+
+// a store that never happens but that the compiler cannot prove never happens
+__device__ __forceinline__ void abl_sink(uint32_t v, int32_t *dst) {
+    if (v == 0x9e3779b9u) *dst = (int32_t)v;
+}
+
 struct PreSmem {
     ViewCam cams[GS_CAM_CHUNK];
     float strata[GS_CAM_CHUNK][BIN_SUB];  // depth-stratum boundaries of the staged views (PreEmit::strata)
@@ -140,7 +159,8 @@ __device__ __forceinline__ void project_splat(const DevCfg &c, const ViewCam &ca
     out.radius = (int32_t)rad;
     out.meta = GS_META_VISIBLE;
     float3 rgb;
-    if (COLOUR == 2) rgb = eval_sh(c.deg, sh, sh_view_dir(m, cam.campos), out.meta);
+    if (COLOUR == 2 && (ABL & ABL_SH)) rgb = make_float3(0.5f, 0.5f, 0.5f);
+    else if (COLOUR == 2) rgb = eval_sh(c.deg, sh, sh_view_dir(m, cam.campos), out.meta);
     else if (COLOUR == 1) rgb = make_float3(rgb_in[0], rgb_in[1], rgb_in[2]);
     else rgb = make_float3(0.f, 0.f, 0.f);   // COLOUR == 0: k_sh_colour fills the three colour words of the record
     // Tight binning.  A pixel can only receive this Gaussian if alpha = o*G >= 1/255, i.e. log2 G >= -log2(255 o).
@@ -197,7 +217,7 @@ k_preprocess(const DevCfg c, const DevInputs in, float4 *__restrict__ rec0, floa
     const int RS = (c.M == MS || sh_raw16) ? c.M * 3 : 49;   // floats per staged row (3 M = 75 for PF3plat: 11 t mod 32, conflict-free)
     constexpr bool HAS_SH = COLOUR == 2;
     bool bulk = false;
-    if (HAS_SH) {
+    if (HAS_SH && !(ABL & ABL_SH)) {
         const float *src = in.shs + ((size_t)scene * c.P + g0) * c.M * 3;
         if (c.M == MS) {
             const uint32_t bytes = (uint32_t)n * c.M * 12u;
@@ -251,6 +271,15 @@ k_preprocess(const DevCfg c, const DevInputs in, float4 *__restrict__ rec0, floa
             cov3d_from_scale_rot(s, c.scale_modifier, q, c6);
         }
     }
+    // (knock-out build only) the first chunk's cameras are staged before the SH barrier instead of between a pair of their own
+    constexpr bool EARLY_CAMS = (ABL & ABL_BAR) && HAS_SH;
+    if (EARLY_CAMS) {
+        const int nv = min(GS_CAM_CHUNK, c.VPS);
+        load_view_cams(c, scene * c.VPS, nv, sm->cams);
+        if (emit.strata && !emit.strata_per_tile)
+            for (int t = tid; t < nv * BIN_SUB; t += PRE_THREADS)
+                sm->strata[t / BIN_SUB][t % BIN_SUB] = emit.strata[(size_t)(scene * c.VPS) * BIN_SUB + t];
+    }
     if (HAS_SH) {
         cp_async_wait<0>();  // this thread's share of the strided copy (no-op on the other paths)
         __syncthreads();     // barrier init (bulk) or the copies (fallbacks) visible to everyone
@@ -277,12 +306,14 @@ k_preprocess(const DevCfg c, const DevInputs in, float4 *__restrict__ rec0, floa
 
     for (int v0 = 0; v0 < c.VPS; v0 += GS_CAM_CHUNK) {
         const int nv = min(GS_CAM_CHUNK, c.VPS - v0);
-        __syncthreads();
-        load_view_cams(c, scene * c.VPS + v0, nv, sm->cams);
-        if (emit.strata && !emit.strata_per_tile)
-            for (int t = tid; t < nv * BIN_SUB; t += PRE_THREADS)
-                sm->strata[t / BIN_SUB][t % BIN_SUB] = emit.strata[(size_t)(scene * c.VPS + v0) * BIN_SUB + t];
-        __syncthreads();
+        if (!(EARLY_CAMS && v0 == 0)) {
+            __syncthreads();
+            load_view_cams(c, scene * c.VPS + v0, nv, sm->cams);
+            if (emit.strata && !emit.strata_per_tile)
+                for (int t = tid; t < nv * BIN_SUB; t += PRE_THREADS)
+                    sm->strata[t / BIN_SUB][t % BIN_SUB] = emit.strata[(size_t)(scene * c.VPS + v0) * BIN_SUB + t];
+            __syncthreads();
+        }
         if (!active) continue;
         for (int vi = 0; vi < nv; vi++) {
             const int v = scene * c.VPS + v0 + vi;
@@ -290,19 +321,40 @@ k_preprocess(const DevCfg c, const DevInputs in, float4 *__restrict__ rec0, floa
             Splat sp;
             project_splat<COLOUR>(c, sm->cams[vi], mean, c6, opac, sh_s + (size_t)tid * RS,
                                   COLOUR == 1 ? in.colors_precomp + o * 3 : nullptr, sp);
-            if (sp.radius > 0) {
+            // fused speculative emission: nothing reads the rects afterwards (k_emit_buckets and the strata learning, their
+            // readers, run on the other paths only)
+            const bool fused = emit.counters && emit.bucket;
+            // (the knock-out builds keep every store and emission of the exact path, where the capacities they run on are learned)
+            const bool abl_spec = ABL && fused;
+            if ((ABL & ABL_REC) && abl_spec && sp.radius > 0) {
+                abl_sink(__float_as_uint(sp.r0.x) ^ __float_as_uint(sp.r0.y) ^ __float_as_uint(sp.r0.z) ^ __float_as_uint(sp.r0.w) ^
+                             __float_as_uint(sp.r1.x) ^ __float_as_uint(sp.r1.y) ^ __float_as_uint(sp.r1.z) ^ __float_as_uint(sp.r1.w) ^
+                             __float_as_uint(sp.r2.x) ^ __float_as_uint(sp.r2.y) ^ __float_as_uint(sp.r2.z),
+                         radii + o);
+            } else if (COLOUR != 0 && !((ABL & ABL_REC) && abl_spec)) {
+                // Every pair's records are stored, zeros for a pair that is not visible (nothing reads those): a warp then
+                // writes whole 32-byte sectors.  Skipping the invisible lanes left sectors half written, which L2 has to
+                // complete with a DRAM read before it can write them back.
+                const bool vis = sp.radius > 0;
+                const float4 z = make_float4(0.f, 0.f, 0.f, 0.f);
+                rec0[o] = vis ? sp.r0 : z;
+                rec1[o] = vis ? sp.r1 : z;
+                rec2[o] = vis ? sp.r2 : z;
+            } else if (COLOUR == 0 && sp.radius > 0) {
+                // the colour words (rec1.zw, rec2.x) belong to k_sh_colour, which may be running right now
                 rec0[o] = sp.r0;
-                if (COLOUR != 0) {
-                    rec1[o] = sp.r1;
-                    rec2[o] = sp.r2;
-                } else {   // the colour words (rec1.zw, rec2.x) belong to k_sh_colour, which may be running right now
-                    *reinterpret_cast<float2 *>(&rec1[o]) = make_float2(sp.r1.x, sp.r1.y);
-                    reinterpret_cast<float *>(&rec2[o])[1] = sp.r2.y;
-                    reinterpret_cast<float2 *>(&rec2[o])[1] = make_float2(sp.r2.z, sp.r2.w);
-                }
+                *reinterpret_cast<float2 *>(&rec1[o]) = make_float2(sp.r1.x, sp.r1.y);
+                reinterpret_cast<float *>(&rec2[o])[1] = sp.r2.y;
+                reinterpret_cast<float2 *>(&rec2[o])[1] = make_float2(sp.r2.z, sp.r2.w);
             }
-            radii[o] = sp.radius;
-            rects[o] = sp.rect;
+            if ((ABL & ABL_RRM) && abl_spec) {
+                abl_sink((uint32_t)sp.radius ^ sp.meta ^ sp.rect.x ^ ((uint32_t)sp.rect.y << 8) ^ ((uint32_t)sp.rect.z << 16) ^
+                             ((uint32_t)sp.rect.w << 24),
+                         radii + o);
+            } else {
+                radii[o] = sp.radius;
+                if (!fused) rects[o] = sp.rect;
+            }
             // Hand this Gaussian to every (view, tile) list it joins.  Exact path: count it (RED.ADD, no return;
             // k_emit_buckets appends it later, once the offsets are known).  Speculative path: append it now to the
             // tile's fixed-capacity sub-bucket; an entry beyond the capacity is dropped and the overflow is detected
@@ -326,12 +378,13 @@ k_preprocess(const DevCfg c, const DevInputs in, float4 *__restrict__ rec0, floa
                     // candidates in row-major order of the rectangle; (cx, cy) walks it without the integer division
                     // that t / w cost per candidate (the emission loop is a large share of this kernel's instructions)
                     int cx = sp.rect.x, cy = sp.rect.y;
+                    uint32_t abl_acc = 0;
                     for (int t0 = 0; t0 < nt; t0 += EMIT_BATCH) {
                         bool ok[EMIT_BATCH];
                         uint32_t slot[EMIT_BATCH];
 #pragma unroll
                         for (int k = 0; k < EMIT_BATCH; k++) {
-                            ok[k] = cy < (int)sp.rect.w && gs_tile_reached(sp.r0, sp.r1, sp.r2, cx, cy);
+                            ok[k] = cy < (int)sp.rect.w && ((ABL & ABL_TESTS) || gs_tile_reached(sp.r0, sp.r1, sp.r2, cx, cy));
                             const uint32_t tile = tbase + (uint32_t)(cy * c.gx + cx);
                             // per-tile boundaries (clouds whose tiles each see a narrow depth range): the candidate
                             // tile's own eight floats decide the stratum
@@ -342,6 +395,11 @@ k_preprocess(const DevCfg c, const DevInputs in, float4 *__restrict__ rec0, floa
                                 cy++;
                             }
                         }
+                        if (ABL & ABL_EMIT) {
+#pragma unroll
+                            for (int k = 0; k < EMIT_BATCH; k++) abl_acc ^= ok[k] ? slot[k] : 0u;
+                            continue;
+                        }
                         flush_pending();
                         pend_key = ((uint64_t)__float_as_uint(sp.r2.y) << 32) | (uint32_t)i;
 #pragma unroll
@@ -351,6 +409,7 @@ k_preprocess(const DevCfg c, const DevInputs in, float4 *__restrict__ rec0, floa
                             if (ok[k]) pend_pos[k] = atomicAdd(&emit.counters[(size_t)slot[k] * BIN_PAD], 1u);
                         }
                     }
+                    if (ABL & ABL_EMIT) abl_sink(abl_acc, radii + o);
                 } else {
                     for (int ty = sp.rect.y; ty < (int)sp.rect.w; ty++)
                         for (int tx = sp.rect.x; tx < (int)sp.rect.z; tx++)
@@ -358,7 +417,7 @@ k_preprocess(const DevCfg c, const DevInputs in, float4 *__restrict__ rec0, floa
                                 atomicAdd(&emit.counters[(size_t)((tbase + (uint32_t)(ty * c.gx + tx)) * BIN_SUB + sub) * BIN_PAD], 1u);
                 }
             }
-            meta[o] = (uint8_t)sp.meta;
+            if (!((ABL & ABL_RRM) && abl_spec)) meta[o] = (uint8_t)sp.meta;
         }
     }
     flush_pending();

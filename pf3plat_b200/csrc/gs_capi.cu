@@ -55,25 +55,6 @@ struct GrowBuf {
     }
 };
 
-enum { STRATA_UNKNOWN = 0, STRATA_TRIAL = 1, STRATA_ON = 2, STRATA_OFF = 3 };
-
-// speculative bucket capacities learned from the previous forward of the same shape (0 = none yet)
-struct SpecState {
-    int V = 0, ntiles = 0;
-    uint32_t sub_cap = 0;     // capacity of one of a tile's BIN_SUB sub-buckets
-    uint32_t tile_limit = 0;  // list length the tile sort is launched for
-    // Depth strata (gs_binning.cu).  UNKNOWN: no boundaries for this shape yet.  TRIAL: boundaries learned by the
-    // last exact-path call, capacities still those of index % BIN_SUB sub-buckets -> the next speculative call
-    // tries strata with doubled capacities.  ON: strata with capacities learned from stratified counts.
-    // OFF: the trial overflowed (a tile whose depths crowd into one stratum): this shape stays on whole-tile sorts.
-    int strata_state = STRATA_UNKNOWN;
-    // Which boundaries `strata` holds: one row per view (octiles of the view's depths), or -- for shapes whose
-    // per-view trial overflowed: tiles that each see a narrow depth range, e.g. PF3plat's pixel-aligned Gaussians on
-    // a smooth surface -- one row per (view, tile), learned from the exact call's sorted lists and refreshed by the
-    // stratum sort of every call (two tables, swapped on success).
-    int strata_per_tile = 0, want_per_tile = 0, tile_tab = 0;
-};
-
 struct GsContext {
     // Private stream-ordered pool: saved state (records, lists, image planes) and scratch -- never the device's default
     // pool.  Blocks freed by gs_saved_free stay cached for the next calls (pool_follow: a periodic, bounded trim);
@@ -85,20 +66,12 @@ struct GsContext {
     GrowBuf host_stage;    // device mirror of host buffers (gs_render_host)
     uint32_t *d_word = nullptr;  // device alias of h_word (mapped pinned memory)
     uint32_t *h_word = nullptr;  // pinned, written by the device: [0] tile instances, [1] longest tile list, [2] largest sub-counter, [3] overflow
-    // What earlier forwards of a SHAPE (views, tiles, Gaussians per scene, scenes) taught: speculative bucket capacities,
-    // the strata state machine and its boundary tables.  A context remembers SHAPE_SLOTS shapes (least recently used one
-    // evicted), so a caller that alternates shapes -- context and target views of a training step, training and validation
-    // batches -- keeps every one of them on the speculative path; `spec` / `strata` point at the slot of the running call.
+    // the shapes earlier forwards taught (gs_bin_policy.h), each with its boundary tables: [V][BIN_SUB] (or two tables
+    // of [V*tiles][BIN_SUB]) stratum boundaries + histogram scratch
     static constexpr int SHAPE_SLOTS = 4;
-    struct ShapeSlot {
-        int key_V = -1, key_ntiles = -1, key_P = -1, key_S = -1;
-        uint64_t last_use = 0;
-        SpecState spec;
-        GrowBuf strata;   // [V][BIN_SUB] (or two tables of [V*tiles][BIN_SUB]) stratum boundaries + histogram scratch
-    } slots[SHAPE_SLOTS];
+    ShapeSlot slots[SHAPE_SLOTS];
+    GrowBuf strata_tabs[SHAPE_SLOTS];
     uint64_t use_counter = 0;
-    SpecState *spec = &slots[0].spec;
-    GrowBuf *strata = &slots[0].strata;
     cudaEvent_t ev_pre = nullptr;   // "preprocess done" (speculative path: lets the radii copy start early)
     cudaEvent_t ev_info = nullptr;  // "binning verdict copied to the host"
     // gs_render_host's split pipeline: k_sh_colour pulls the SH block out of the caller's pinned buffer on aux_stream while
@@ -108,16 +81,8 @@ struct GsContext {
     // gs_render_host: radii are final once the forward's mid-way sync has passed, so their copy to the host
     // overlaps binning + compositing on a side stream
     cudaStream_t copy_stream = nullptr;
-    void *host_radii_dst = nullptr;
-    size_t host_radii_bytes = 0;
-    // gs_render_host: the SH block arrives in feed_chunks pieces on the copy stream; piece k (Gaussians
-    // [feed_begin[k], feed_begin[k+1])) is complete once feed_ev[k] has fired, and preprocess runs piece by piece
-    // behind them, so all but the last piece of preprocess hides under the host-to-device transfer
     static constexpr int FEED_MAX = 8;
-    int feed_chunks = 0;
-    bool sh_zero_copy = false;         // gs_render_host: in->shs is the device alias of the caller's pinned buffer (preprocess pulls it over PCIe)
-    int feed_begin[FEED_MAX + 1] = {};
-    cudaEvent_t feed_ev[FEED_MAX] = {};
+    cudaEvent_t feed_ev[FEED_MAX] = {};   // gs_render_host: piece k of the SH block has landed (HostFeed)
     GsStats stats{};
     bool profiling = false;
     cudaEvent_t ev[GS_NUM_STAGES + 1][2]{};
@@ -215,34 +180,6 @@ size_t saved_layout(GsSaved *s, const DevCfg &c, unsigned char *base) {
     return off;
 }
 
-// Capacities for the next forward of this shape: 30 % headroom over what this one needed.
-// Capacities are quantised and sticky: a capacity that still fits and is not more than 1.5x what is needed is kept, so
-// that a cloud that moves a little every step (training) asks the memory pool for the SAME block sizes call after call
-// (with capacities re-derived every call, the varying sizes of a jittered cloud defeat the pool's reuse and the
-// mapping of new blocks costs more than the kernels).
-inline uint32_t sticky_capacity(uint32_t need, uint32_t current) {
-    need = (need + 63u) & ~63u;
-    return (current >= need && (uint64_t)current * 2 <= (uint64_t)need * 3) ? current : need;
-}
-
-void learn_capacities(GsContext *ctx, const DevCfg &c, uint32_t max_tile, uint32_t max_sub) {
-    const bool same_shape = ctx->spec->V == c.V && ctx->spec->ntiles == c.ntiles;
-    const uint32_t sub_cap = sticky_capacity(max_sub + max_sub * 3 / 10 + 16, same_shape ? ctx->spec->sub_cap : 0u);
-    const uint32_t limit = sticky_capacity(max_tile + max_tile / 10 + 32, same_shape ? ctx->spec->tile_limit : 0u);
-    if (limit > BIN_SMEM_CAP || (uint64_t)sub_cap * BIN_SUB * c.V * c.ntiles > 0xffffffffull) {
-        ctx->spec->sub_cap = 0;  // lists too long for the shared-memory sort (or offsets beyond 32 bits): exact path
-        return;
-    }
-    if (ctx->spec->V != c.V || ctx->spec->ntiles != c.ntiles) {
-        ctx->spec->strata_state = STRATA_UNKNOWN;
-        ctx->spec->strata_per_tile = ctx->spec->want_per_tile = 0;
-    }
-    ctx->spec->V = c.V;
-    ctx->spec->ntiles = c.ntiles;
-    ctx->spec->sub_cap = sub_cap;
-    ctx->spec->tile_limit = limit;
-}
-
 }  // namespace
 
 extern "C" int gs_context_create(GsContext **out) {
@@ -280,7 +217,7 @@ extern "C" void gs_context_destroy(GsContext *ctx) {
     ctx->per_gaussian.release();
     ctx->sort.release();
     ctx->host_stage.release();
-    for (auto &sl : ctx->slots) sl.strata.release();
+    for (auto &b : ctx->strata_tabs) b.release();
     if (ctx->copy_stream) cudaStreamDestroy(ctx->copy_stream);
     if (ctx->aux_stream) cudaStreamDestroy(ctx->aux_stream);
     if (ctx->ev_alloc) cudaEventDestroy(ctx->ev_alloc);
@@ -306,20 +243,8 @@ extern "C" int gs_context_trim(GsContext *ctx) {
 }
 
 namespace {
-// Memory policy of the context's private pool.  Freed blocks stay in the pool (release threshold = never, set at creation):
-// every automatic scheme tried released memory that the very next calls mapped again, and both directions are expensive
-// (mapping is paid per MB, and releasing at a synchronisation stalls that call and the next):
-//   * threshold = scratch + 1.25 x saved state, updated every call: a shape that is still settling (exact call, strata
-//     trial, re-learned capacities, the backward's accumulator growing the scratch) changes its block sizes from call to call
-//     -- forward + backward at the C4 size stalled for several steps, with hiccups well after that;
-//   * the same once settled: the usual training loop (`out = render(...)`, rebinding `out`) keeps the previous step's saved
-//     state alive until the new forward has returned -- room for one meant mapping a second every step;
-//   * room for two: the reference's decoder makes a call per view plus one per view for depth, and autograd holds all their
-//     saved states until the backward (12 at PF3plat's 2 x 3 views): mapping again every step; following the pool's
-//     high-water mark fixed that but left hiccups whenever a capacity changed.
-// So, like the caching allocator of the host framework, the pool only gives memory back when asked (gs_context_trim /
-// rasterizer.trim_memory, gs_context_destroy) -- or here, every 256 calls, when it holds more than twice the high-water
-// mark of what those 256 calls had handed out at any one time (a one-off large batch does not pin its memory for ever).
+// Memory policy of the context's private pool (DESIGN.md 4): freed blocks stay cached; every 256 calls the pool is
+// trimmed when it holds more than twice the high-water mark of what those calls had handed out at any one time.
 void pool_follow(GsContext *ctx) {
     if (++ctx->calls_since_peak_reset < 256) return;
     ctx->calls_since_peak_reset = 0;
@@ -377,398 +302,313 @@ extern "C" void gs_saved_free(GsContext *ctx, GsSaved *saved, void *stream) {
     delete saved;
 }
 
-extern "C" int gs_forward(GsContext *ctx, const GsConfig *cfg, const GsInputs *in, const GsOutputs *out,
-                          GsSaved **saved_out, void *stream) {
+namespace {
+// gs_render_host's per-call feed of the forward (null for device-resident inputs)
+struct HostFeed {
+    bool sh_zero_copy;   // in->shs is the device alias of the caller's pinned buffer (preprocess pulls it over PCIe)
+    // the SH block arrives in `chunks` pieces on the copy stream, piece k (Gaussians [begin[k], begin[k+1])) complete
+    // once ctx->feed_ev[k] has fired: preprocess runs piece by piece behind them (DESIGN.md 5.6)
+    int chunks, begin[GsContext::FEED_MAX + 1];
+    void *radii_dst;     // host buffer the radii ([V*P] int32) are copied to on the copy stream as soon as they are final
+};
+
+#define FWD_OK(call) do { const int rc_ = (call); if (rc_ != GS_OK) return rc_; } while (0)
+#define FWD_CUDA(call, what) \
+    do { const cudaError_t e_ = (call); if (e_ != cudaSuccess) return gs_set_cuda_error(e_, what, __FILE__, __LINE__); } while (0)
+
+// One forward call: what its speculative attempt and its exact path share, and what they leave for the commit.
+struct FwdCall {
+    GsContext *ctx;
+    DevCfg c;
+    DevInputs di;
+    const GsOutputs *out;
+    cudaStream_t st;
+    const HostFeed *feed;
+    void *radii_dst; size_t radii_bytes;  // gs_render_host: host destination of the radii
+    uint32_t tuning;
+    int pre_variant, composite_variant;   // launch_preprocess / launch_composite_fwd variants
+    bool split_colour, merge_sort;        // k_sh_colour on the aux stream; GS_TUNE_STRATA_MERGE_SORT
+    // scratch: rects[n] | counters | cursors | verdict words | sub-bucket offsets | tile_start | tile_n
+    ushort4 *rects;
+    uint32_t *tile_counts, *cursor, *verdict_acc, *sub_offsets, *tile_start, *tile_n;
+    size_t ctr_bytes;
+    GsSaved *s;
+    bool colour_pending;   // k_sh_colour is (or may still be) writing into s->rec1 / s->rec2 on the aux stream
+    int64_t D;
+    size_t list_bytes;
+    int start_colour();
+    int speculate(SpecState &spec, const BinShape &shape, const BinPlan &plan, GrowBuf &tabs, bool *committed);
+    int exact(SpecState &spec, const BinShape &shape, GrowBuf &tabs);
+    size_t scratch_layout(unsigned char *base) {
+        size_t off = 0;
+        const size_t n = (size_t)c.V * c.P, nvt = (size_t)c.V * c.ntiles;
+        auto take = [&](size_t bytes) {
+            unsigned char *p = base ? base + off : nullptr;
+            off += align256(bytes);
+            return reinterpret_cast<uint32_t *>(p);
+        };
+        ctr_bytes = align256(bin_counter_bytes(c));
+        rects = reinterpret_cast<ushort4 *>(take(n * 8));
+        tile_counts = take(ctr_bytes);
+        cursor = take(ctr_bytes);
+        verdict_acc = take(256);  // directly behind the cursors: one memset clears both
+        sub_offsets = take(nvt * BIN_SUB * 4);
+        tile_start = take(nvt * 4);
+        tile_n = take(nvt * 4);
+        return off;
+    }
+
+    int fail(int code) {
+        if (colour_pending) cudaStreamWaitEvent(st, ctx->ev_colour, 0);   // the free below is ordered on `st`
+        gs_saved_free(ctx, s, st);
+        return code;
+    }
+    // the tile-instance list lives in its own stream-ordered allocation (s->point_list stays null when it fails)
+    cudaError_t alloc_list(size_t bytes) {
+        void *p = nullptr;
+        const cudaError_t e = cudaMallocFromPoolAsync(&p, bytes, ctx->pool, st);
+        if (e == cudaSuccess) s->point_list = static_cast<uint32_t *>(p);
+        list_bytes = bytes;
+        return e;
+    }
+    template <class F> int timed(int stage, F launch) {
+        StageTimer t(ctx, stage, st);
+        return launch();
+    }
+    // the compositor needs the colour words: from here on `st` itself is ordered behind the colour kernel
+    int composite() {
+        if (colour_pending) {
+            colour_pending = false;
+            FWD_CUDA(cudaStreamWaitEvent(st, ctx->ev_colour, 0), "cudaStreamWaitEvent(colour)");
+        }
+        return timed(GS_STAGE_COMPOSITE, [&] { return launch_composite_fwd(c, *s, out->color, out->depth, st, composite_variant); });
+    }
+};
+
+// gs_render_host's split pipeline: k_sh_colour writes the colour words of s->rec1 / s->rec2 on the aux stream, behind
+// everything enqueued on `st` so far (the caller's uploads of means and cameras, the allocation of the records)
+int FwdCall::start_colour() {
+    const char *setup = "split colour pipeline setup";
+    if (!ctx->aux_stream) FWD_CUDA(cudaStreamCreateWithFlags(&ctx->aux_stream, cudaStreamNonBlocking), setup);
+    if (!ctx->ev_alloc) FWD_CUDA(cudaEventCreateWithFlags(&ctx->ev_alloc, cudaEventDisableTiming), setup);
+    if (!ctx->ev_colour) FWD_CUDA(cudaEventCreateWithFlags(&ctx->ev_colour, cudaEventDisableTiming), setup);
+    FWD_CUDA(cudaEventRecord(ctx->ev_alloc, st), setup);
+    FWD_CUDA(cudaStreamWaitEvent(ctx->aux_stream, ctx->ev_alloc, 0), setup);
+    {
+        StageTimer t(ctx, GS_STAGE_SH_COLOUR, ctx->aux_stream);
+        FWD_OK(launch_sh_colour(c, di, s->rec1, s->rec2, nullptr, ctx->aux_stream));
+    }
+    const cudaError_t e = cudaEventRecord(ctx->ev_colour, ctx->aux_stream);
+    if (e != cudaSuccess) cudaStreamSynchronize(ctx->aux_stream);   // the caller frees the records
+    FWD_CUDA(e, "cudaEventRecord(colour)");
+    colour_pending = true;
+    return GS_OK;
+}
+
+// Speculative attempt (DESIGN.md 5.2): the host reads the verdict only after the tile sort and the compositor have been
+// enqueued.  *committed = false after an overflow: the results are discarded and the call is redone on the exact path.
+int FwdCall::speculate(SpecState &spec, const BinShape &shape, const BinPlan &plan, GrowBuf &tabs, bool *committed) {
+    const size_t slots = (size_t)c.V * c.ntiles * BIN_SUB;
+    const float *strata_tab = plan.read_tab < 0 ? nullptr : static_cast<float *>(tabs.p) + (size_t)plan.read_tab * slots;
+    float *strata_next = plan.write_tab < 0 ? nullptr : static_cast<float *>(tabs.p) + (size_t)plan.write_tab * slots;
+    FWD_OK(ctx->sort.reserve(slots * plan.sub_cap * 8, 1.0, ctx->pool, st));
+    FWD_CUDA(alloc_list(slots * plan.sub_cap * 4), "cudaMallocAsync(point_list)");
+    FWD_CUDA(cudaMemsetAsync(cursor, 0, ctr_bytes + 256, st), "cudaMemsetAsync(cursors)");
+    const PreEmit emit{plan.fused_emit ? cursor : nullptr, static_cast<uint64_t *>(ctx->sort.p), plan.sub_cap,
+                       strata_tab, plan.per_tile};
+    {
+        StageTimer t(ctx, GS_STAGE_PREPROCESS, st);
+        const int pieces = feed ? feed->chunks : 0;
+        for (int k = 0; k < (pieces ? pieces : 1); k++) {
+            if (pieces) FWD_CUDA(cudaStreamWaitEvent(st, ctx->feed_ev[k], 0), "cudaStreamWaitEvent(feed)");
+            FWD_OK(launch_preprocess(c, di, s->rec0, s->rec1, s->rec2, s->meta, out->radii, rects, emit, st,
+                                     pieces ? feed->begin[k] : 0, pieces ? feed->begin[k + 1] : -1, pre_variant));
+        }
+    }
+    if (!plan.fused_emit)
+        FWD_OK(timed(GS_STAGE_BIN_EMIT, [&] {
+            return bin_emit_fast(c, 1, s->rec0, s->rec1, s->rec2, rects, nullptr, plan.sub_cap, strata_tab,
+                                 plan.per_tile, cursor, ctx->sort.p, st);
+        }));
+    // gs_render_host: the radii leave as soon as they are final; on the stratified path only after the sort, whose verdict
+    // store into host memory would otherwise queue behind the 16 MB of radii on the PCIe link
+    auto start_radii_copy = [&]() -> int {
+        if (!radii_dst) return GS_OK;
+        const char *what = "early radii copy";
+        if (!ctx->ev_pre) FWD_CUDA(cudaEventCreateWithFlags(&ctx->ev_pre, cudaEventDisableTiming), what);
+        FWD_CUDA(cudaEventRecord(ctx->ev_pre, st), what);
+        FWD_CUDA(cudaStreamWaitEvent(ctx->copy_stream, ctx->ev_pre, 0), what);
+        FWD_CUDA(cudaMemcpyAsync(radii_dst, out->radii, radii_bytes, cudaMemcpyDeviceToHost, ctx->copy_stream), what);
+        return GS_OK;
+    };
+    if (!plan.strata) FWD_OK(start_radii_copy());
+    // the verdict goes straight into mapped pinned memory, marked by ev_info: from k_spec_check on the whole-tile path,
+    // from the stratum sort's last CTA on the stratified path
+    if (!ctx->ev_info) FWD_CUDA(cudaEventCreateWithFlags(&ctx->ev_info, cudaEventDisableTiming), "cudaEventCreate");
+    if (!plan.strata) {
+        FWD_OK(timed(GS_STAGE_BIN_SCAN, [&] { return bin_spec_check(c, plan.sub_cap, spec.tile_limit, cursor, ctx->d_word, st); }));
+        FWD_CUDA(cudaEventRecord(ctx->ev_info, st), "read back binning info");
+    }
+    {
+        StageTimer t(ctx, GS_STAGE_BIN_SORT, st);
+        if (plan.strata) {
+            FWD_OK(bin_sort_strata(c, plan.sub_cap, cursor, ctx->sort.p, s->point_list, s->ranges, verdict_acc,
+                                   ctx->d_word, st, merge_sort, s->rec2, strata_next));
+            FWD_CUDA(cudaEventRecord(ctx->ev_info, st), "read back binning info");
+            FWD_OK(start_radii_copy());
+        } else {
+            FWD_OK(bin_sort_spec(c, plan.sub_cap, spec.tile_limit, cursor, ctx->sort.p, s->point_list, s->ranges, st));
+        }
+    }
+    FWD_OK(composite());
+    FWD_CUDA(cudaEventSynchronize(ctx->ev_info), "cudaEventSynchronize");  // the one host sync of the forward (verification only)
+    bool release_sort;
+    *committed = learn_speculative(spec, shape, plan, ctx->h_word, ctx->sort.bytes, tuning, &release_sort);
+    if (release_sort) {   // stream-ordered
+        ctx->sort.pooled ? cudaFreeAsync(ctx->sort.p, st) : cudaFree(ctx->sort.p);
+        ctx->sort = GrowBuf{};
+    }
+    if (*committed) {
+        D = (int64_t)ctx->h_word[0];
+        // k_preprocess, [k_sh_colour,] [k_emit_buckets,] [k_spec_check,] tile sort, k_composite_fwd
+        ctx->stats.kernel_launches = (plan.strata ? 3 : 4) + (plan.fused_emit ? 0 : 1) + (split_colour ? 1 : 0);
+        ctx->stats.max_tile_list = (int32_t)ctx->h_word[1];
+        ctx->stats.speculative = plan.strata ? 2 : 1;
+        return GS_OK;
+    }
+    ctx->stats.overflow_redos++;
+    if (radii_dst) cudaStreamSynchronize(ctx->copy_stream);
+    cudaFreeAsync(s->point_list, st);
+    s->point_list = nullptr;
+    for (bool &valid : ctx->ev_valid) valid = false;
+    return GS_OK;
+}
+
+// Exact path: count, scan, the one host sync, emit, sort; then boundaries for the coming speculative calls.
+int FwdCall::exact(SpecState &spec, const BinShape &shape, GrowBuf &tabs) {
+    ctx->stats.speculative = 0;
+    {
+        StageTimer t(ctx, GS_STAGE_PREPROCESS, st);
+        FWD_CUDA(cudaMemsetAsync(tile_counts, 0, bin_counter_bytes(c), st), "cudaMemsetAsync(tile_counts)");
+        const PreEmit emit{tile_counts, nullptr, 0, nullptr, 0};  // sub-bucket = index % BIN_SUB
+        for (int k = 0; feed && k < feed->chunks; k++)  // gs_render_host: every piece of the SH block must have landed
+            FWD_CUDA(cudaStreamWaitEvent(st, ctx->feed_ev[k], 0), "cudaStreamWaitEvent(feed)");
+        FWD_OK(launch_preprocess(c, di, s->rec0, s->rec1, s->rec2, s->meta, out->radii, rects, emit, st, 0, -1, pre_variant));
+        ctx->stats.kernel_launches += (c.P > 0);
+    }
+    uint32_t max_count;   // longest tile list
+    bool fast;            // shared-memory sort
+    int learn;            // boundaries to learn
+    {
+        StageTimer t(ctx, GS_STAGE_BIN_SCAN, st);
+        // the scan kernel stores its three result words straight into pinned host memory (no copy-engine hop)
+        FWD_OK(bin_tile_scan(c, tile_counts, sub_offsets, tile_start, tile_n, ctx->d_word, st));
+        FWD_CUDA(cudaStreamSynchronize(st), "read back num_rendered");
+        D = (int64_t)ctx->h_word[0];
+        max_count = ctx->h_word[1];
+        fast = bin_fits_fast_path(max_count) && !(tuning & GS_TUNE_FORCE_RADIX_BINNING);
+        learn = learn_exact(spec, shape, (size_t)c.V * c.P, max_count, ctx->h_word[2], fast, tuning);
+        if (radii_dst)  // preprocess has completed: radii can leave now
+            FWD_CUDA(cudaMemcpyAsync(radii_dst, out->radii, radii_bytes, cudaMemcpyDeviceToHost, ctx->copy_stream),
+                     "cudaMemcpyAsync(radii)");
+        if (D > 0x7fffffffll) return gs_set_error(GS_ERR_OVERFLOW, "more than 2^31-1 tile instances");
+        FWD_CUDA(alloc_list((size_t)(D > 0 ? D : 1) * 4), "cudaMallocAsync(point_list)");
+    }
+    FWD_OK(ctx->sort.reserve(bin_scratch_bytes(c, D, fast), 1.25, ctx->pool, st));
+    FWD_OK(timed(GS_STAGE_BIN_EMIT, [&] {
+        return fast ? bin_emit_fast(c, D, s->rec0, s->rec1, s->rec2, rects, sub_offsets, 0, nullptr, 0,
+                                    cursor, ctx->sort.p, st)
+                    : bin_sort_fallback(c, D, s->rec0, s->rec1, s->rec2, rects, ctx->sort.p, ctx->sort.bytes,
+                                        s->point_list, s->ranges, st);
+    }));
+    if (fast)
+        FWD_OK(timed(GS_STAGE_BIN_SORT, [&] {
+            return bin_sort_fast(c, max_count, tile_start, tile_n, ctx->sort.p, s->point_list, s->ranges, st);
+        }));
+    ctx->stats.kernel_launches += 1 + (D > 0 ? 1 : 0) + 1;  // scan, emit, tile sort (fallback: 3 + CUB's)
+    ctx->stats.max_tile_list = (int32_t)max_count;
+    FWD_OK(composite());
+    ctx->stats.kernel_launches += 1;
+    if (learn != LEARN_NONE) {
+        FWD_OK(tabs.reserve(bin_strata_bytes(c), 1.0, ctx->pool, st));
+        FWD_OK(learn == LEARN_PER_TILE ? bin_learn_tile_strata(c, s->point_list, s->ranges, s->rec2, static_cast<float *>(tabs.p), st)
+                                       : bin_learn_strata(c, rects, s->rec2, tabs.p, st));
+        start_trial(spec);
+        ctx->stats.kernel_launches += learn == LEARN_PER_TILE ? 1 : 2;  // k_tile_octiles | k_depth_hist, k_strata_from_hist
+    }
+    return GS_OK;
+}
+#undef FWD_OK
+#undef FWD_CUDA
+
+int forward(GsContext *ctx, const GsConfig *cfg, const GsInputs *in, const GsOutputs *out, GsSaved **saved_out,
+            cudaStream_t st, const HostFeed *feed) {
     if (saved_out) *saved_out = nullptr;
     if (!ctx || !out) return gs_set_error(GS_ERR_INVALID, "null context/outputs");
     int rc = validate(cfg, in);
     if (rc != GS_OK) return rc;
     if (!out->color || (cfg->P > 0 && !out->radii)) return gs_set_error(GS_ERR_INVALID, "color/radii outputs missing");
     if ((cfg->flags & GS_FLAG_DEPTH) && !out->depth) return gs_set_error(GS_ERR_INVALID, "GS_FLAG_DEPTH needs out->depth");
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    const DevCfg c = make_dev_cfg(cfg);
-    const DevInputs di = make_dev_inputs(in);
+    FwdCall f{};
+    f.ctx = ctx; f.c = make_dev_cfg(cfg); f.di = make_dev_inputs(in); f.out = out; f.st = st; f.feed = feed;
+    const DevCfg &c = f.c;
     const size_t n = (size_t)c.V * c.P;
-    {   // this shape's slot: what its earlier calls taught (GsContext::ShapeSlot); least recently used slot on a miss
-        GsContext::ShapeSlot *hit = nullptr, *lru = &ctx->slots[0];
-        for (auto &sl : ctx->slots) {
-            if (sl.key_V == c.V && sl.key_ntiles == c.ntiles && sl.key_P == c.P && sl.key_S == c.S) hit = &sl;
-            if (sl.last_use < lru->last_use) lru = &sl;
-        }
-        if (!hit) {
-            hit = lru;
-            hit->spec = SpecState{};   // (the slot's boundary buffer is kept and re-filled by the exact call)
-            hit->key_V = c.V; hit->key_ntiles = c.ntiles; hit->key_P = c.P; hit->key_S = c.S;
-        }
-        hit->last_use = ++ctx->use_counter;
-        ctx->spec = &hit->spec;
-        ctx->strata = &hit->strata;
-    }
-    // gs_render_host with a pinned SH block: geometry-only preprocess here, colours by k_sh_colour on a second stream
-    const bool split_colour = ctx->sh_zero_copy && !(cfg->tuning & GS_TUNE_NO_SPLIT_COLOUR) && n > 0 && sh_colour_supported(c, di);
-    const int pre_low = ((cfg->tuning & GS_TUNE_PRE_OCC6) ? 1 : 0) | (((cfg->tuning & GS_TUNE_PRE_SH_RAW16) || ctx->sh_zero_copy) ? 2 : 0) |
-                        (split_colour ? 4 : 0);
-    for (bool &v : ctx->ev_valid) v = false;
+    const BinShape shape{c.V, c.ntiles, c.P, c.S};
+    const int slot = pick_slot(ctx->slots, GsContext::SHAPE_SLOTS, ctx->use_counter, shape);
+    SpecState &spec = ctx->slots[slot].spec;
+    GrowBuf &tabs = ctx->strata_tabs[slot];
+    const BinPlan plan = plan_binning(spec, shape, n, tabs.p != nullptr, cfg->tuning);
+
+    // kernel variants (gs_render_host with a pinned SH block: geometry-only preprocess, colours in k_sh_colour)
+    f.tuning = cfg->tuning;
+    const bool zero_copy = feed && feed->sh_zero_copy;
+    f.split_colour = zero_copy && !(f.tuning & GS_TUNE_NO_SPLIT_COLOUR) && n > 0 && sh_colour_supported(c, f.di);
+    f.pre_variant = ((f.tuning & GS_TUNE_PRE_OCC6) ? 1 : 0) | (((f.tuning & GS_TUNE_PRE_SH_RAW16) || zero_copy) ? 2 : 0) |
+                    (f.split_colour ? 4 : 0);
+    f.composite_variant = (f.tuning & GS_TUNE_FWD_WS) ? 2 : 0;
+    f.merge_sort = (f.tuning & GS_TUNE_STRATA_MERGE_SORT) != 0;
+    f.radii_dst = feed && ctx->copy_stream ? feed->radii_dst : nullptr;
+    f.radii_bytes = n * 4;
+    for (bool &valid : ctx->ev_valid) valid = false;
     ctx->stats.kernel_launches = 0;
 
-    // ---- per-call scratch: rects[n] | counters | cursors | verdict words | sub-bucket offsets | tile_start | tile_n ----
-    const size_t nvt = (size_t)c.V * c.ntiles;
-    const size_t ctr_bytes = align256(bin_counter_bytes(c));
-    const size_t pg_bytes = align256(n * 8) + 2 * ctr_bytes + 256 + align256(nvt * BIN_SUB * 4) + 2 * align256(nvt * 4);
-    rc = ctx->per_gaussian.reserve(pg_bytes, 1.0, ctx->pool, st);
+    rc = ctx->per_gaussian.reserve(f.scratch_layout(nullptr), 1.0, ctx->pool, st);
     if (rc != GS_OK) return rc;
-    unsigned char *pg = static_cast<unsigned char *>(ctx->per_gaussian.p);
-    ushort4 *rects = reinterpret_cast<ushort4 *>(pg);
-    pg += align256(n * 8);
-    uint32_t *tile_counts = reinterpret_cast<uint32_t *>(pg);
-    pg += ctr_bytes;
-    uint32_t *cursor = reinterpret_cast<uint32_t *>(pg);
-    pg += ctr_bytes;
-    uint32_t *verdict_acc = reinterpret_cast<uint32_t *>(pg);  // directly behind the cursors: one memset clears both
-    pg += 256;
-    uint32_t *sub_offsets = reinterpret_cast<uint32_t *>(pg);
-    pg += align256(nvt * BIN_SUB * 4);
-    uint32_t *tile_start = reinterpret_cast<uint32_t *>(pg);
-    pg += align256(nvt * 4);
-    uint32_t *tile_n = reinterpret_cast<uint32_t *>(pg);
-
+    f.scratch_layout(static_cast<unsigned char *>(ctx->per_gaussian.p));
     // ---- saved state: geometry / image planes now, the tile-instance list once its length is known ----
-    GsSaved *s = new (std::nothrow) GsSaved();
+    GsSaved *s = f.s = new (std::nothrow) GsSaved();   // value-initialised: all zero
     if (!s) return gs_set_error(GS_ERR_OOM, "host allocation failed");
-    memset(s, 0, sizeof(*s));
-    {
-        const size_t bytes = saved_layout(s, c, nullptr);
-        unsigned char *block = nullptr;
-        cudaError_t e = cudaMallocFromPoolAsync(reinterpret_cast<void **>(&block), bytes, ctx->pool, st);
-        if (e != cudaSuccess) {
-            delete s;
-            return gs_set_cuda_error(e, "cudaMallocAsync(saved)", __FILE__, __LINE__);
-        }
-        saved_layout(s, c, block);
-        s->base = block;
-        s->bytes = bytes;
+    s->bytes = saved_layout(s, c, nullptr);
+    const cudaError_t e = cudaMallocFromPoolAsync(&s->base, s->bytes, ctx->pool, st);
+    if (e != cudaSuccess) {
+        delete s;
+        return gs_set_cuda_error(e, "cudaMallocAsync(saved)", __FILE__, __LINE__);
     }
-    bool colour_pending = false;   // k_sh_colour is (or may still be) writing into s->rec1 / s->rec2 on the aux stream
-    auto fail = [&](int code) {
-        if (colour_pending) cudaStreamWaitEvent(st, ctx->ev_colour, 0);   // the free below is ordered on `st`
-        gs_saved_free(ctx, s, stream);
-        return code;
-    };
-    if (split_colour) {
-        cudaError_t e = cudaSuccess;
-        if (!ctx->aux_stream) e = cudaStreamCreateWithFlags(&ctx->aux_stream, cudaStreamNonBlocking);
-        if (e == cudaSuccess && !ctx->ev_alloc) e = cudaEventCreateWithFlags(&ctx->ev_alloc, cudaEventDisableTiming);
-        if (e == cudaSuccess && !ctx->ev_colour) e = cudaEventCreateWithFlags(&ctx->ev_colour, cudaEventDisableTiming);
-        // everything enqueued on `st` so far -- the caller's uploads of means and cameras, the allocation of the records --
-        // precedes the colour kernel
-        if (e == cudaSuccess) e = cudaEventRecord(ctx->ev_alloc, st);
-        if (e == cudaSuccess) e = cudaStreamWaitEvent(ctx->aux_stream, ctx->ev_alloc, 0);
-        if (e != cudaSuccess) return fail(gs_set_cuda_error(e, "split colour pipeline setup", __FILE__, __LINE__));
-        {
-            StageTimer t(ctx, GS_STAGE_SH_COLOUR, ctx->aux_stream);
-            rc = launch_sh_colour(c, di, s->rec1, s->rec2, nullptr, ctx->aux_stream);
-        }
-        if (rc != GS_OK) return fail(rc);
-        colour_pending = true;
-        e = cudaEventRecord(ctx->ev_colour, ctx->aux_stream);
-        if (e != cudaSuccess) {
-            cudaStreamSynchronize(ctx->aux_stream);
-            colour_pending = false;
-            return fail(gs_set_cuda_error(e, "cudaEventRecord(colour)", __FILE__, __LINE__));
-        }
-    }
-    // the compositor needs the colour words: called right before each of its launches
-    auto join_colour = [&]() -> cudaError_t {
-        if (!colour_pending) return cudaSuccess;
-        colour_pending = false;   // from here on `st` itself is ordered behind the colour kernel
-        return cudaStreamWaitEvent(st, ctx->ev_colour, 0);
-    };
+    saved_layout(s, c, static_cast<unsigned char *>(s->base));
+    if (f.split_colour && (rc = f.start_colour()) != GS_OK) return f.fail(rc);
 
-    // ---- speculative-capacity forward: no count/scan passes and no mid-pipeline bubble ----
-    // The tile instances go straight into fixed-capacity sub-buckets sized from the previous forward of this shape;
-    // a one-CTA kernel right after preprocess checks that nothing overflowed, and the host reads its verdict only
-    // after the tile sort and the compositor have been enqueued behind it.  On overflow the results are discarded
-    // and the call is redone below on the exact path (which re-learns the capacities).
-    const bool speculate = ctx->spec->sub_cap > 0 && ctx->spec->V == c.V && ctx->spec->ntiles == c.ntiles && n > 0 &&
-                           !(cfg->tuning & (GS_TUNE_FORCE_RADIX_BINNING | GS_TUNE_NO_SPECULATION));
-    if (speculate) {
-        bool strata = (ctx->spec->strata_state == STRATA_TRIAL || ctx->spec->strata_state == STRATA_ON) &&
-                      !(cfg->tuning & GS_TUNE_NO_STRATA) && ctx->strata->p != nullptr;
-        uint32_t sub_cap = ctx->spec->sub_cap;
-        if (strata && ctx->spec->strata_state == STRATA_TRIAL) {
-            // capacities were learned unstratified: the trial runs on doubled ones -- if the kernels' 32-bit bucket
-            // offsets still hold them (learn_capacities checked the undoubled value only)
-            // A cloud whose tiles each see a narrow depth range (PF3plat's pixel-aligned Gaussians on a smooth surface)
-            // puts a tile's whole list into one or two of the per-view strata: the trial must be able to hold a whole
-            // list per stratum, memory permitting (the capacities learned from it are what later calls allocate).
-            // (Sizing the trial for a WHOLE tile list per stratum -- so that clouds whose tiles each see a narrow depth
-            // range, like PF3plat's pixel-aligned Gaussians, stay stratified -- was dropped: such a shape
-            // then sorts one or two 1 600-key strata per tile with a single warp each, slower than the whole-tile merge
-            // sort + verdict kernel it falls back to.  Per-TILE boundaries are the fix.)
-            uint32_t trial = sub_cap * 2;
-            if (trial > BIN_STRATUM_CAP) trial = BIN_STRATUM_CAP;
-            if ((uint64_t)trial * BIN_SUB * nvt > 0xffffffffull) strata = false;
-            else sub_cap = trial;
-        }
-        if (strata && sub_cap > BIN_STRATUM_CAP) sub_cap = BIN_STRATUM_CAP;
-        const int per_tile = strata ? ctx->spec->strata_per_tile : 0;
-        const size_t tab_floats = nvt * BIN_SUB;  // one per-tile table
-        float *tab0 = static_cast<float *>(ctx->strata->p);
-        const float *strata_tab = !strata ? nullptr : (per_tile ? tab0 + (size_t)ctx->spec->tile_tab * tab_floats : tab0);
-        float *strata_next = (strata && per_tile) ? tab0 + (size_t)(ctx->spec->tile_tab ^ 1) * tab_floats : nullptr;
-        const size_t slots = nvt * BIN_SUB;
-        rc = ctx->sort.reserve(slots * sub_cap * 8, 1.0, ctx->pool, st);
-        if (rc != GS_OK) return fail(rc);
-        cudaError_t e = cudaMallocFromPoolAsync(reinterpret_cast<void **>(&s->point_list), slots * sub_cap * 4, ctx->pool, st);
-        if (e != cudaSuccess) {
-            s->point_list = nullptr;
-            return fail(gs_set_cuda_error(e, "cudaMallocAsync(point_list)", __FILE__, __LINE__));
-        }
-        e = cudaMemsetAsync(cursor, 0, ctr_bytes + 256, st);
-        if (e != cudaSuccess) return fail(gs_set_cuda_error(e, "cudaMemsetAsync(cursors)", __FILE__, __LINE__));
-        // Appending from inside preprocess touches the buckets of ALL views at once; far beyond L2 size those 8-byte
-        // appends turn into partial-sector DRAM writes, so big bucket sets (C4) are filled by the view-major
-        // k_emit_buckets instead.  The bound sits above the 50 MB L2 of an H100 because C2's buckets, which exceed it,
-        // are still filled faster by the fused appends on an H100 (README.md; `bench.py --tuning 4` forces k_emit_buckets).
-        const bool fused_emit = slots * sub_cap * 8 <= ((size_t)96 << 20) && !(cfg->tuning & GS_TUNE_SEPARATE_EMIT);
-        {
-            StageTimer t(ctx, GS_STAGE_PREPROCESS, st);
-            const PreEmit emit{fused_emit ? cursor : nullptr, static_cast<uint64_t *>(ctx->sort.p), sub_cap, strata_tab, per_tile};
-            if (ctx->feed_chunks > 0) {
-                for (int k = 0; k < ctx->feed_chunks && rc == GS_OK; k++) {
-                    e = cudaStreamWaitEvent(st, ctx->feed_ev[k], 0);
-                    if (e != cudaSuccess) return fail(gs_set_cuda_error(e, "cudaStreamWaitEvent(feed)", __FILE__, __LINE__));
-                    rc = launch_preprocess(c, di, s->rec0, s->rec1, s->rec2, s->meta, out->radii, rects, emit, st,
-                                           ctx->feed_begin[k], ctx->feed_begin[k + 1], pre_low);
-                }
-            } else {
-                rc = launch_preprocess(c, di, s->rec0, s->rec1, s->rec2, s->meta, out->radii, rects, emit, st, 0, -1, pre_low);
-            }
-            if (rc != GS_OK) return fail(rc);
-        }
-        if (!fused_emit) {
-            StageTimer t(ctx, GS_STAGE_BIN_EMIT, st);
-            rc = bin_emit_fast(c, 1, s->rec0, s->rec1, s->rec2, rects, nullptr, sub_cap, strata_tab, per_tile, cursor, ctx->sort.p, st);
-            if (rc != GS_OK) return fail(rc);
-        }
-        // gs_render_host: the radii leave for the host on the copy stream as soon as they are final -- after preprocess
-        // on the whole-tile path; after the sort on the stratified path, whose last CTA stores the verdict into host
-        // memory (a store that would otherwise sit behind the 16 MB of radii on the PCIe link)
-        auto start_radii_copy = [&]() -> cudaError_t {
-            if (!(ctx->host_radii_dst && ctx->copy_stream)) return cudaSuccess;
-            cudaError_t ee = cudaSuccess;
-            if (!ctx->ev_pre) ee = cudaEventCreateWithFlags(&ctx->ev_pre, cudaEventDisableTiming);
-            if (ee == cudaSuccess) ee = cudaEventRecord(ctx->ev_pre, st);
-            if (ee == cudaSuccess) ee = cudaStreamWaitEvent(ctx->copy_stream, ctx->ev_pre, 0);
-            if (ee == cudaSuccess)
-                ee = cudaMemcpyAsync(ctx->host_radii_dst, out->radii, ctx->host_radii_bytes, cudaMemcpyDeviceToHost,
-                                     ctx->copy_stream);
-            return ee;
-        };
-        if (!strata && (e = start_radii_copy()) != cudaSuccess)
-            return fail(gs_set_cuda_error(e, "early radii copy", __FILE__, __LINE__));
-        // The verdict (overflow flag, counts) follows from the cursors alone.  Whole-tile path: one tiny kernel right
-        // after preprocess; stratified path: the sort's CTAs add it up themselves and the last one publishes it.  Either
-        // way it is stored straight into mapped pinned memory (an in-stream D2H copy would queue behind the 16 MB
-        // radii copy of gs_render_host in the copy engine) and marked with an event, and the remaining kernels are
-        // enqueued BEFORE the host waits on that event: the caller gets control back (to enqueue its next call) while
-        // the GPU is still busy.
-        if (!ctx->ev_info) {
-            e = cudaEventCreateWithFlags(&ctx->ev_info, cudaEventDisableTiming);
-            if (e != cudaSuccess) return fail(gs_set_cuda_error(e, "cudaEventCreate", __FILE__, __LINE__));
-        }
-        if (!strata) {
-            StageTimer t(ctx, GS_STAGE_BIN_SCAN, st);
-            rc = bin_spec_check(c, sub_cap, ctx->spec->tile_limit, cursor, ctx->d_word, st);
-            if (rc != GS_OK) return fail(rc);
-            e = cudaEventRecord(ctx->ev_info, st);
-            if (e != cudaSuccess) return fail(gs_set_cuda_error(e, "read back binning info", __FILE__, __LINE__));
-        }
-        {
-            StageTimer t(ctx, GS_STAGE_BIN_SORT, st);
-            if (strata) {
-                rc = bin_sort_strata(c, sub_cap, cursor, ctx->sort.p, s->point_list, s->ranges, verdict_acc, ctx->d_word, st,
-                                     (cfg->tuning & GS_TUNE_STRATA_MERGE_SORT) != 0, s->rec2, strata_next);
-                if (rc == GS_OK && (e = cudaEventRecord(ctx->ev_info, st)) != cudaSuccess)
-                    return fail(gs_set_cuda_error(e, "read back binning info", __FILE__, __LINE__));
-                if (rc == GS_OK && (e = start_radii_copy()) != cudaSuccess)
-                    return fail(gs_set_cuda_error(e, "early radii copy", __FILE__, __LINE__));
-            } else {
-                rc = bin_sort_spec(c, sub_cap, ctx->spec->tile_limit, cursor, ctx->sort.p, s->point_list, s->ranges, st);
-            }
-            if (rc != GS_OK) return fail(rc);
-        }
-        if ((e = join_colour()) != cudaSuccess) return fail(gs_set_cuda_error(e, "cudaStreamWaitEvent(colour)", __FILE__, __LINE__));
-        {
-            StageTimer t(ctx, GS_STAGE_COMPOSITE, st);
-            rc = launch_composite_fwd(c, *s, out->color, out->depth, st, (cfg->tuning & GS_TUNE_FWD_WS) ? 2 : 0);
-            if (rc != GS_OK) return fail(rc);
-        }
-        e = cudaEventSynchronize(ctx->ev_info);  // the one host sync of the forward (verification only)
-        if (e != cudaSuccess) return fail(gs_set_cuda_error(e, "cudaEventSynchronize", __FILE__, __LINE__));
-        if (ctx->h_word[3] == 0) {
-            const int64_t D = (int64_t)ctx->h_word[0];
-            if (strata) {
-                // capacities for the next call from the stratified counts just measured; a stratum beyond the small
-                // sort's capacity sends this shape back to whole-tile sorts (via one exact-path call)
-                uint32_t next = sticky_capacity(ctx->h_word[2] + ctx->h_word[2] * 3 / 10 + 16,
-                                                ctx->spec->strata_state == STRATA_ON ? sub_cap : 0u);
-                if (next > BIN_STRATUM_CAP && ctx->h_word[2] + ctx->h_word[2] / 10 <= BIN_STRATUM_CAP) next = BIN_STRATUM_CAP;  // 10 % headroom still fits
-                if (next > BIN_STRATUM_CAP) {
-                    ctx->spec->strata_state = STRATA_OFF;
-                    ctx->spec->sub_cap = 0;
-                } else {
-                    if (ctx->spec->strata_state == STRATA_TRIAL && ctx->sort.bytes > 2 * (slots * (size_t)next * 8) + ((size_t)8 << 20)) {
-                        // the trial's generous buckets are not needed again: give the block back (stream-ordered)
-                        if (ctx->sort.pooled) cudaFreeAsync(ctx->sort.p, st);
-                        else cudaFree(ctx->sort.p);
-                        ctx->sort.p = nullptr;
-                        ctx->sort.bytes = 0;
-                    }
-                    ctx->spec->strata_state = STRATA_ON;
-                    ctx->spec->sub_cap = next;
-                    if (per_tile) ctx->spec->tile_tab ^= 1;  // the sort wrote the next call's boundaries into the other table
-                }
-            } else {
-                learn_capacities(ctx, c, ctx->h_word[1], ctx->h_word[2]);
-            }
-            s->D = D;
-            s->P = c.P; s->S = c.S; s->V = c.V; s->H = c.H; s->W = c.W;
-            s->flags = c.flags;
-            s->has_sh = in->shs != nullptr;
-            s->has_scales = in->scales != nullptr;
-            ctx->stats.kernel_launches = (strata ? 3 : 4) + (fused_emit ? 0 : 1) + (split_colour ? 1 : 0);  // k_preprocess, [k_sh_colour,] [k_emit_buckets], [k_spec_check,] tile sort, k_composite_fwd
-            ctx->stats.max_tile_list = (int32_t)ctx->h_word[1];
-            ctx->stats.num_rendered = D;
-            ctx->stats.num_visible = -1;
-            ctx->stats.saved_bytes = (int64_t)(s->bytes + slots * sub_cap * 4);
-            pool_follow(ctx);
-            ctx->stats.speculative = strata ? 2 : 1;
-            if (saved_out) *saved_out = s;
-            else gs_saved_free(ctx, s, stream);
-            return GS_OK;
-        }
-        // overflow: some sub-bucket or tile list outgrew its capacity.  Results are invalid; redo exactly.
-        ctx->stats.overflow_redos++;
-        ctx->spec->sub_cap = 0;
-        if (strata) {
-            if (ctx->spec->strata_state == STRATA_TRIAL && !per_tile && !(cfg->tuning & GS_TUNE_NO_TILE_STRATA)) {
-                // the per-view boundaries crowd some tile into one stratum: the exact redo below learns per-tile ones
-                ctx->spec->want_per_tile = 1;
-                ctx->spec->strata_state = STRATA_UNKNOWN;
-            } else {
-                ctx->spec->strata_state = ctx->spec->strata_state == STRATA_TRIAL ? STRATA_OFF : STRATA_UNKNOWN;
-            }
-        }
-        if (ctx->host_radii_dst && ctx->copy_stream) cudaStreamSynchronize(ctx->copy_stream);
-        cudaFreeAsync(s->point_list, st);
-        s->point_list = nullptr;
-        for (bool &v : ctx->ev_valid) v = false;
-    }
-    ctx->stats.speculative = 0;
+    bool committed = false;
+    if (plan.speculate && (rc = f.speculate(spec, shape, plan, tabs, &committed)) != GS_OK) return f.fail(rc);
+    if (!committed && (rc = f.exact(spec, shape, tabs)) != GS_OK) return f.fail(rc);
 
-    {
-        StageTimer t(ctx, GS_STAGE_PREPROCESS, st);
-        cudaError_t e = cudaMemsetAsync(tile_counts, 0, bin_counter_bytes(c), st);
-        if (e != cudaSuccess) return fail(gs_set_cuda_error(e, "cudaMemsetAsync(tile_counts)", __FILE__, __LINE__));
-        const PreEmit emit{tile_counts, nullptr, 0, nullptr, 0};  // exact path: sub-bucket = index % BIN_SUB
-        for (int k = 0; k < ctx->feed_chunks; k++) {  // gs_render_host: every piece of the SH block must have landed
-            e = cudaStreamWaitEvent(st, ctx->feed_ev[k], 0);
-            if (e != cudaSuccess) return fail(gs_set_cuda_error(e, "cudaStreamWaitEvent(feed)", __FILE__, __LINE__));
-        }
-        rc = launch_preprocess(c, di, s->rec0, s->rec1, s->rec2, s->meta, out->radii, rects, emit, st, 0, -1, pre_low);
-        if (rc != GS_OK) return fail(rc);
-        ctx->stats.kernel_launches += (c.P > 0);
-    }
-
-    int64_t D = 0;
-    uint32_t max_count = 0;
-    {
-        StageTimer t(ctx, GS_STAGE_BIN_SCAN, st);
-        // the scan kernel stores its three result words straight into pinned host memory (no copy-engine hop)
-        rc = bin_tile_scan(c, tile_counts, sub_offsets, tile_start, tile_n, ctx->d_word, st);
-        if (rc != GS_OK) return fail(rc);
-        cudaError_t e = cudaStreamSynchronize(st);  // the one host sync of the (exact) forward
-        if (e != cudaSuccess) return fail(gs_set_cuda_error(e, "read back num_rendered", __FILE__, __LINE__));
-        D = (int64_t)ctx->h_word[0];
-        max_count = ctx->h_word[1];
-        learn_capacities(ctx, c, max_count, ctx->h_word[2]);
-        if (ctx->host_radii_dst && ctx->copy_stream) {  // preprocess has completed: radii can leave now
-            e = cudaMemcpyAsync(ctx->host_radii_dst, out->radii, ctx->host_radii_bytes, cudaMemcpyDeviceToHost,
-                                ctx->copy_stream);
-            if (e != cudaSuccess) return fail(gs_set_cuda_error(e, "cudaMemcpyAsync(radii)", __FILE__, __LINE__));
-        }
-        if (D > 0x7fffffffll) return fail(gs_set_error(GS_ERR_OVERFLOW, "more than 2^31-1 tile instances"));
-        // the list lives in its own stream-ordered allocation (sized exactly)
-        e = cudaMallocFromPoolAsync(reinterpret_cast<void **>(&s->point_list), (size_t)(D > 0 ? D : 1) * 4, ctx->pool, st);
-        if (e != cudaSuccess) {
-            s->point_list = nullptr;
-            return fail(gs_set_cuda_error(e, "cudaMallocAsync(point_list)", __FILE__, __LINE__));
-        }
-        s->D = D;
-    }
-    const bool fast = bin_fits_fast_path(max_count) && !(cfg->tuning & GS_TUNE_FORCE_RADIX_BINNING);
-    rc = ctx->sort.reserve(bin_scratch_bytes(c, D, fast), 1.25, ctx->pool, st);
-    if (rc != GS_OK) return fail(rc);
-    {
-        StageTimer t(ctx, GS_STAGE_BIN_EMIT, st);
-        if (fast)
-            rc = bin_emit_fast(c, D, s->rec0, s->rec1, s->rec2, rects, sub_offsets, 0, nullptr, 0, cursor, ctx->sort.p, st);
-        else
-            rc = bin_sort_fallback(c, D, s->rec0, s->rec1, s->rec2, rects, ctx->sort.p, ctx->sort.bytes, s->point_list,
-                                   s->ranges, st);
-        if (rc != GS_OK) return fail(rc);
-    }
-    if (fast) {
-        StageTimer t(ctx, GS_STAGE_BIN_SORT, st);
-        rc = bin_sort_fast(c, max_count, tile_start, tile_n, ctx->sort.p, s->point_list, s->ranges, st);
-        if (rc != GS_OK) return fail(rc);
-    }
-    ctx->stats.kernel_launches += 1 + (D > 0 ? 1 : 0) + 1;  // scan, emit, tile sort (fallback: 3 + CUB's)
-    ctx->stats.max_tile_list = (int32_t)max_count;
-
-    {
-        cudaError_t e = join_colour();
-        if (e != cudaSuccess) return fail(gs_set_cuda_error(e, "cudaStreamWaitEvent(colour)", __FILE__, __LINE__));
-    }
-    {
-        StageTimer t(ctx, GS_STAGE_COMPOSITE, st);
-        rc = launch_composite_fwd(c, *s, out->color, out->depth, st, (cfg->tuning & GS_TUNE_FWD_WS) ? 2 : 0);
-        if (rc != GS_OK) return fail(rc);
-        ctx->stats.kernel_launches += 1;
-    }
-
-    // Depth-stratum boundaries for the coming speculative calls, from this call's depths (off this call's critical
-    // path: queued behind the compositor).  STRATA_OFF is sticky for the shape.
-    if (fast && ctx->spec->sub_cap > 0 && ctx->spec->strata_state != STRATA_OFF && !(cfg->tuning & GS_TUNE_NO_STRATA) && n > 0) {
-        rc = ctx->strata->reserve(bin_strata_bytes(c), 1.0, ctx->pool, st);
-        if (rc != GS_OK) return fail(rc);
-        if (ctx->spec->want_per_tile) {
-            ctx->spec->tile_tab = 0;
-            rc = bin_learn_tile_strata(c, s->point_list, s->ranges, s->rec2, static_cast<float *>(ctx->strata->p), st);
-        } else {
-            rc = bin_learn_strata(c, rects, s->rec2, ctx->strata->p, st);
-        }
-        if (rc != GS_OK) return fail(rc);
-        ctx->spec->strata_state = STRATA_TRIAL;
-        ctx->spec->strata_per_tile = ctx->spec->want_per_tile;
-        ctx->stats.kernel_launches += ctx->spec->want_per_tile ? 1 : 2;  // k_tile_octiles | k_depth_hist, k_strata_from_hist
-    }
-
+    s->D = f.D;
     s->P = c.P; s->S = c.S; s->V = c.V; s->H = c.H; s->W = c.W;
     s->flags = c.flags;
     s->has_sh = in->shs != nullptr;
     s->has_scales = in->scales != nullptr;
-    ctx->stats.num_rendered = D;
+    ctx->stats.num_rendered = f.D;
     ctx->stats.num_visible = -1;
-    ctx->stats.saved_bytes = (int64_t)(s->bytes + (size_t)(D > 0 ? D : 1) * 4);
+    ctx->stats.saved_bytes = (int64_t)(s->bytes + f.list_bytes);
     pool_follow(ctx);
-    if (saved_out) {
-        *saved_out = s;
-    } else {
-        gs_saved_free(ctx, s, stream);
-    }
+    if (saved_out) *saved_out = s;
+    else gs_saved_free(ctx, s, st);
     return GS_OK;
+}
+}  // namespace
+
+extern "C" int gs_forward(GsContext *ctx, const GsConfig *cfg, const GsInputs *in, const GsOutputs *out,
+                          GsSaved **saved_out, void *stream) {
+    return forward(ctx, cfg, in, out, saved_out, static_cast<cudaStream_t>(stream), nullptr);
 }
 
 extern "C" int gs_backward(GsContext *ctx, const GsConfig *cfg, const GsInputs *in, const GsSaved *saved,
@@ -907,6 +747,7 @@ extern "C" int gs_render_host(GsContext *ctx, const GsConfig *cfg, const GsInput
     // The SH block is most of the bytes (C2: 150 of 170 MB).  A single scene's block goes over in pieces on the copy
     // stream, each marked with an event, and gs_forward runs preprocess piece by piece behind them.
     const size_t sh_row = (size_t)cfg->M * 12;
+    HostFeed feed{};
     int pieces = 0;
     if (in->shs && !sh_alias && cfg->S == 1 && (size_t)cfg->P * sh_row >= ((size_t)16 << 20)) {
         // more pieces overlap more of preprocess with the transfer (scripts/ab_e2e.py compares piece counts)
@@ -940,14 +781,14 @@ extern "C" int gs_render_host(GsContext *ctx, const GsConfig *cfg, const GsInput
             GS_CUDA_OK(cudaMemcpyAsync(base + sh_off + (size_t)g * sh_row, reinterpret_cast<const char *>(in->shs) + (size_t)g * sh_row,
                                        (size_t)(g1 - g) * sh_row, cudaMemcpyHostToDevice, ctx->copy_stream));
             GS_CUDA_OK(cudaEventRecord(ctx->feed_ev[k], ctx->copy_stream));
-            ctx->feed_begin[k] = g;
-            ctx->feed_begin[k + 1] = g1;
+            feed.begin[k] = g;
+            feed.begin[k + 1] = g1;
         }
         pieces = k;
     }
-    ctx->feed_chunks = pieces;
-    ctx->host_radii_dst = (out->radii && VP) ? out->radii : nullptr;
-    ctx->host_radii_bytes = VP * 4;
+    feed.chunks = pieces;
+    feed.sh_zero_copy = sh_alias != nullptr;
+    feed.radii_dst = (out->radii && VP) ? out->radii : nullptr;
     dout.color = reinterpret_cast<float *>(base + out_off);
     dout.radii = reinterpret_cast<int32_t *>(base + out_off + align256(px * 12));
     dout.depth = (cfg->flags & GS_FLAG_DEPTH) ? reinterpret_cast<float *>(base + out_off + align256(px * 12) + align256(VP * 4))
@@ -962,11 +803,7 @@ extern "C" int gs_render_host(GsContext *ctx, const GsConfig *cfg, const GsInput
     void *depth_alias = direct && dout.depth ? device_alias(out->depth) : nullptr;
     if (color_alias) dout.color = static_cast<float *>(color_alias);
     if (depth_alias) dout.depth = static_cast<float *>(depth_alias);
-    ctx->sh_zero_copy = sh_alias != nullptr;
-    rc = gs_forward(ctx, &dc, &din, &dout, nullptr, stream);
-    ctx->sh_zero_copy = false;
-    ctx->host_radii_dst = nullptr;
-    ctx->feed_chunks = 0;
+    rc = forward(ctx, &dc, &din, &dout, nullptr, st, &feed);
     if (rc != GS_OK) {
         // nothing of ours may still be reading the caller's buffers (the colour kernel pulls out of them) once we return
         if (ctx->aux_stream) cudaStreamSynchronize(ctx->aux_stream);

@@ -14,6 +14,7 @@
 #include <stdint.h>
 
 #include "../../include/gsplat_b200.h"
+#include "gs_bin_policy.h"
 #include "gs_det.cuh"
 
 #define GS_TILE 16
@@ -81,8 +82,6 @@ int launch_sh_colour(const DevCfg &c, const DevInputs &in, float4 *rec1, float4 
 int launch_mark_visible(const DevCfg &c, const float *means3D, uint8_t *present, cudaStream_t st);
 
 // binning (gs_binning.cu)
-#define BIN_SMEM_CAP 8192  // longest tile list the shared-memory merge sort takes (256 threads x 32 keys)
-#define BIN_SUB 8          // sub-counters per (view, tile), selected by Gaussian index & (BIN_SUB-1)
 #define BIN_PAD 8          // uint32 stride between counters: one counter per 32-byte L2 sector
 size_t bin_counter_bytes(const DevCfg &c);
 int bin_tile_scan(const DevCfg &c, const uint32_t *counters, uint32_t *offsets, uint32_t *tile_start, uint32_t *tile_n,
@@ -107,7 +106,6 @@ int bin_learn_tile_strata(const DevCfg &c, const uint32_t *point_list, const uin
 // depth strata: per-view octiles of the depths of the binned Gaussians (weighted by their tile count), for the NEXT call
 size_t bin_strata_bytes(const DevCfg &c);          // strata table [V][BIN_SUB] floats + histogram scratch
 int bin_learn_strata(const DevCfg &c, const ushort4 *rects, const float4 *rec2, void *strata_buf, cudaStream_t st);
-constexpr uint32_t BIN_STRATUM_CAP = 2048;         // longest sub-bucket k_stratum_sort handles (128 threads x 16 keys)
 int bin_sort_spec(const DevCfg &c, uint32_t sub_cap, uint32_t tile_limit, const uint32_t *cursor, const void *bucket,
                   uint32_t *point_list, uint2 *ranges, cudaStream_t st);
 int bin_sort_fallback(const DevCfg &c, int64_t D, const float4 *rec0, const float4 *rec1, const float4 *rec2,

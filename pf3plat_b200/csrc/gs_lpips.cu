@@ -16,11 +16,15 @@
 //                             TF32): M = pixels of all images, N = Cout, K = 9 Cin.  The backward-data pass is the same
 //                             kernel on weights rotated by 180 degrees with Cin/Cout swapped (packed once), its epilogue
 //                             applying the ReLU mask of the layer below
-//   k_pool / k_unpool_bwd     2x2 max-pool; its backward routes to the first maximum of each window (PyTorch's choice),
-//                             adds the head's gradient of the tap and applies the tap's ReLU mask
+//   k_pool / k_unpool_bwd     2x2 max-pool; its backward routes to the first maximum of each window, or to its last NaN
+//                             (PyTorch's choice), adds the head's gradient of the tap and applies the tap's ReLU mask
 //   k_head_fwd / k_head_bwd   one warp per pixel: channel norms, the lin-weighted squared difference, per-CTA fp64
 //                             partial sums reduced in a fixed order by k_head_final; the backward's closed form below
 // No atomics, no host synchronisation: results are bit-identical from run to run.
+//
+// Non-finite inputs follow PyTorch's rules, so a NaN or Inf pixel gives the image a NaN distance and NaN gradients
+// where autograd has them: ReLU and max-pool propagate NaN (max.NaN), ReLU's backward zeroes the gradient only where
+// act <= 0 (a NaN activation passes it), and the max-pool backward routes to a NaN as described above.
 //
 // Head backward: with s = ||f||, n = f/(s+e), g = dL/dn:  dL/df = (g - n (n.g)(s+e)/s) / (s+e).  At s = 0 the second
 // term's limit is 0 (|n (n.g)(s+e)/s| <= |g| s/(s+e)), so dL/df = g/e there (the derivative of f/(s+e) at f = 0);
@@ -48,6 +52,13 @@ __device__ __forceinline__ float tf32_round(float x) {
     uint32_t r;
     asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
     return __uint_as_float(r);
+}
+
+// max that returns NaN if either operand is NaN (PyTorch's relu and max_pool2d); otherwise the bits of fmaxf
+__device__ __forceinline__ float max_nan(float a, float b) {
+    float r;
+    asm("max.NaN.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b));
+    return r;
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -113,7 +124,7 @@ k_conv0_fwd(const float *__restrict__ in0, const float *__restrict__ in1, int64_
     }
     float4 *dst = reinterpret_cast<float4 *>(out + pix * 64 + cg * 8);
 #pragma unroll
-    for (int o = 0; o < 8; o++) acc[o] = tf32_round(fmaxf(acc[o], 0.f));
+    for (int o = 0; o < 8; o++) acc[o] = tf32_round(max_nan(acc[o], 0.f));
     dst[0] = make_float4(acc[0], acc[1], acc[2], acc[3]);
     dst[1] = make_float4(acc[4], acc[5], acc[6], acc[7]);
 }
@@ -164,7 +175,8 @@ struct ConvArgs {
     const float *in;    // NHWC [img][H][W][Cin], TF32 values
     const float *wp;    // [9 Cin][Cout], TF32 values
     const float *bias;  // [Cout]: forward (bias + ReLU); NULL: backward-data
-    const float *mask;  // backward: NHWC [img][H][W][Cout] activation of the layer below (gradient kept where > 0), or NULL
+    const float *mask;  // backward: NHWC [img][H][W][Cout] activation of the layer below (gradient zeroed where <= 0, so
+                        // a NaN activation passes it), or NULL
     float *out;         // NHWC [img][H][W][Cout]
     int64_t M;          // images * H * W
     int H, W, Cin, Cout;
@@ -287,12 +299,12 @@ __global__ void __launch_bounds__(CV_THREADS, 2) k_conv3x3(const ConvArgs p) {
                 if (m >= p.M) continue;
                 float v0 = acc[i][j][2 * h], v1 = acc[i][j][2 * h + 1];
                 if (p.bias) {
-                    v0 = fmaxf(v0 + bias.x, 0.f);
-                    v1 = fmaxf(v1 + bias.y, 0.f);
-                } else if (p.mask) {
+                    v0 = max_nan(v0 + bias.x, 0.f);
+                    v1 = max_nan(v1 + bias.y, 0.f);
+                } else if (p.mask) {  // ReLU's backward: zero where act <= 0, so a NaN activation passes the gradient
                     const float2 mk = *reinterpret_cast<const float2 *>(p.mask + m * Cout + n);
-                    v0 = mk.x > 0.f ? v0 : 0.f;
-                    v1 = mk.y > 0.f ? v1 : 0.f;
+                    v0 = !(mk.x <= 0.f) ? v0 : 0.f;
+                    v1 = !(mk.y <= 0.f) ? v1 : 0.f;
                 }
                 *reinterpret_cast<float2 *>(p.out + m * Cout + n) = make_float2(tf32_round(v0), tf32_round(v1));
             }
@@ -317,22 +329,24 @@ __global__ void k_pool(const float *__restrict__ in, int nimg, int H, int W, int
     const int64_t img = po / ((int64_t)Wo * Ho);
     const float4 *src = reinterpret_cast<const float4 *>(in) + ((img * H + 2 * yo) * W + 2 * xo) * C4 + c4;
     const float4 a = src[0], b = src[C4], c = src[(int64_t)W * C4], d = src[(int64_t)W * C4 + C4];
-    reinterpret_cast<float4 *>(out)[i] = make_float4(fmaxf(fmaxf(a.x, b.x), fmaxf(c.x, d.x)), fmaxf(fmaxf(a.y, b.y), fmaxf(c.y, d.y)),
-                                                     fmaxf(fmaxf(a.z, b.z), fmaxf(c.z, d.z)), fmaxf(fmaxf(a.w, b.w), fmaxf(c.w, d.w)));
+    reinterpret_cast<float4 *>(out)[i] =
+        make_float4(max_nan(max_nan(a.x, b.x), max_nan(c.x, d.x)), max_nan(max_nan(a.y, b.y), max_nan(c.y, d.y)),
+                    max_nan(max_nan(a.z, b.z), max_nan(c.z, d.z)), max_nan(max_nan(a.w, b.w), max_nan(c.w, d.w)));
 }
 
-// index (0..3, row-major) of the first maximum of a 2x2 window, the element max_pool2d's backward routes to
+// index (0..3, row-major) of the element max_pool2d's backward routes a 2x2 window's gradient to: PyTorch's scan
+// `val > maxval || isnan(val)`, i.e. the first maximum, or the last NaN if the window holds one
 __device__ __forceinline__ int first_max(float a, float b, float c, float d) {
     int k = 0;
     float m = a;
-    if (b > m) { m = b; k = 1; }
-    if (c > m) { m = c; k = 2; }
-    if (d > m) k = 3;
+    if (b > m || b != b) { m = b; k = 1; }
+    if (c > m || c != c) { m = c; k = 2; }
+    if (d > m || d != d) k = 3;
     return k;
 }
 
 // g [img][H][W][C] holds the head's (masked) gradient of the tap; adds the pooled gradient gp [img][H/2][W/2][C]
-// routed to each window's first maximum, under the tap's ReLU mask (act > 0), in place
+// routed by first_max, under the tap's ReLU mask (zero where act <= 0), in place
 __global__ void k_unpool_bwd(const float *__restrict__ act, const float *__restrict__ gp, int nimg, int H, int W, int C,
                              float *__restrict__ g) {
     const int Ho = H / 2, Wo = W / 2, C4 = C / 4;
@@ -351,10 +365,10 @@ __global__ void k_unpool_bwd(const float *__restrict__ act, const float *__restr
     const float4 up = reinterpret_cast<const float4 *>(gp)[((img * Ho + yo) * Wo + xo) * C4 + c4];
     const float4 self = a4[pix * C4 + c4];
     float4 v = reinterpret_cast<float4 *>(g)[i];
-    if (first_max(a.x, b.x, c.x, d.x) == me && self.x > 0.f) v.x = tf32_round(v.x + up.x);
-    if (first_max(a.y, b.y, c.y, d.y) == me && self.y > 0.f) v.y = tf32_round(v.y + up.y);
-    if (first_max(a.z, b.z, c.z, d.z) == me && self.z > 0.f) v.z = tf32_round(v.z + up.z);
-    if (first_max(a.w, b.w, c.w, d.w) == me && self.w > 0.f) v.w = tf32_round(v.w + up.w);
+    if (first_max(a.x, b.x, c.x, d.x) == me && !(self.x <= 0.f)) v.x = tf32_round(v.x + up.x);
+    if (first_max(a.y, b.y, c.y, d.y) == me && !(self.y <= 0.f)) v.y = tf32_round(v.y + up.y);
+    if (first_max(a.z, b.z, c.z, d.z) == me && !(self.z <= 0.f)) v.z = tf32_round(v.z + up.z);
+    if (first_max(a.w, b.w, c.w, d.w) == me && !(self.w <= 0.f)) v.w = tf32_round(v.w + up.w);
     reinterpret_cast<float4 *>(g)[i] = v;
 }
 
@@ -456,10 +470,10 @@ k_head_bwd(const float *__restrict__ f, int N, int i0, int HW, const float *__re
         dot = fmaf(n, gn[k], dot);
     }
     dot = warp_sum(dot);
-    const float proj = s > 0.f ? dot * na / s : 0.f;  // the limit at s = 0 (see the top of the file)
+    const float proj = s == 0.f ? 0.f : dot * na / s;  // the limit at s = 0 (see the top of the file); a NaN s stays NaN
     float *dst = g + ((int64_t)(img - i0) * HW + px) * C + lane;
 #pragma unroll
-    for (int k = 0; k < CPL; k++) dst[32 * k] = a[k] > 0.f ? tf32_round((gn[k] - (a[k] / na) * proj) / na) : 0.f;
+    for (int k = 0; k < CPL; k++) dst[32 * k] = !(a[k] <= 0.f) ? tf32_round((gn[k] - (a[k] / na) * proj) / na) : 0.f;
 }
 
 // ---------------------------------------------------------------------------------------------------------

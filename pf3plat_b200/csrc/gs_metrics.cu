@@ -8,8 +8,10 @@
 namespace {
 
 constexpr int PS_THREADS = 256;
+constexpr int MAX_GRID_YZ = 65535;  // gridDim.y and gridDim.z limit: the batch is launched in chunks of at most this
 
-__device__ __forceinline__ float clip01(float x) { return fminf(fmaxf(x, 0.0f), 1.0f); }
+// torch.clip propagates NaN, so a NaN pixel makes the image's PSNR NaN; fminf/fmaxf alone would clip it to 0
+__device__ __forceinline__ float clip01(float x) { return x != x ? x : fminf(fmaxf(x, 0.0f), 1.0f); }
 
 __global__ void __launch_bounds__(PS_THREADS)
 k_sq_err_partial(const float *__restrict__ gt, const float *__restrict__ pred, int64_t n, float *__restrict__ partial) {
@@ -64,6 +66,12 @@ __global__ void k_psnr_finalize(const float *__restrict__ partial, int nblocks, 
 // One CTA per 32x32 tile of the cropped map and channel: the 42x42 input patch of both images is staged in shared
 // memory once, the separable filter runs on the five moment images out of shared memory, and the per-tile sums are
 // reduced deterministically (fp64, no atomics) by k_ssim_finalize.
+//
+// The moments are taken of x - x0 and y - y0, with (x0, y0) the tile's first map pixel: variance and covariance do
+// not change under a shift, and w*x = w*(x - x0) + x0.  Unshifted, w*(x^2) - (w*x)^2 cancels in fp32 to a spurious
+// variance of ~1e-7 x^2, which against C2 = 9e-4 moved S by ~1e-4 on flat bright regions (scipy's filter, which the
+// reference uses, accumulates in fp64 and has no such error).  The last stage rounds every operation on its own
+// (__f*_rn, no contraction), so that identical images give A1 = B1 and A2 = B2 and hence exactly 1.
 // ---------------------------------------------------------------------------------------------------------
 constexpr int SS_TILE = 32, SS_R = 5, SS_TAPS = 2 * SS_R + 1, SS_IN = SS_TILE + 2 * SS_R, SS_THREADS = 256;
 
@@ -81,12 +89,15 @@ k_ssim_partial(const float *__restrict__ gt, const float *__restrict__ pred, int
     const int ox = (tile % tiles_x) * SS_TILE, oy = (tile / tiles_x) * SS_TILE;  // origin in the cropped map == in the image
     const size_t plane = ((size_t)img * gridDim.y + ch) * (size_t)H * W;
     const float *a = gt + plane, *b = pred + plane;
+    // the shift: the image pixel of map pixel (oy, ox), inside the image (oy < H - 10, ox < W - 10)
+    const size_t centre = (size_t)(oy + SS_R) * W + (ox + SS_R);
+    const float x0 = a[centre], y0 = b[centre];
     for (int e = tid; e < SS_IN * SS_IN; e += SS_THREADS) {
         const int r = e / SS_IN, c = e - r * SS_IN;
         const int iy = oy + r, ix = ox + c;
-        const bool in = iy < H && ix < W;
-        sx[r][c] = in ? a[(size_t)iy * W + ix] : 0.f;
-        sy[r][c] = in ? b[(size_t)iy * W + ix] : 0.f;
+        const bool in = iy < H && ix < W;  // outside the image: read only by map pixels the crop drops
+        sx[r][c] = in ? a[(size_t)iy * W + ix] - x0 : 0.f;
+        sy[r][c] = in ? b[(size_t)iy * W + ix] - y0 : 0.f;
     }
     __syncthreads();
     for (int e = tid; e < SS_IN * SS_TILE; e += SS_THREADS) {
@@ -121,9 +132,15 @@ k_ssim_partial(const float *__restrict__ gt, const float *__restrict__ pred, int
             uyy = fmaf(w, hq[3][r + k][c], uyy);
             uxy = fmaf(w, hq[4][r + k][c], uxy);
         }
-        const float vx = cov_norm * (uxx - ux * ux), vy = cov_norm * (uyy - uy * uy), vxy = cov_norm * (uxy - ux * uy);
-        const float A1 = 2.f * ux * uy + C1, A2 = 2.f * vxy + C2, B1 = ux * ux + uy * uy + C1, B2 = vx + vy + C2;
-        acc += (double)((A1 * A2) / (B1 * B2));
+        // shifted moments: ux, uy are w*(x - x0), w*(y - y0)
+        const float vx = __fmul_rn(cov_norm, __fsub_rn(uxx, __fmul_rn(ux, ux)));
+        const float vy = __fmul_rn(cov_norm, __fsub_rn(uyy, __fmul_rn(uy, uy)));
+        const float vxy = __fmul_rn(cov_norm, __fsub_rn(uxy, __fmul_rn(ux, uy)));
+        const float mx = __fadd_rn(ux, x0), my = __fadd_rn(uy, y0);
+        const float A1 = __fadd_rn(__fmul_rn(__fmul_rn(2.f, mx), my), C1);
+        const float B1 = __fadd_rn(__fadd_rn(__fmul_rn(mx, mx), __fmul_rn(my, my)), C1);
+        const float A2 = __fadd_rn(__fmul_rn(2.f, vxy), C2), B2 = __fadd_rn(__fadd_rn(vx, vy), C2);
+        acc += (double)__fdiv_rn(__fmul_rn(A1, A2), __fmul_rn(B1, B2));
     }
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
@@ -162,8 +179,12 @@ extern "C" GS_API int gs_psnr(const float *ground_truth, const float *predicted,
     if (batch == 0) return GS_OK;
     const int blocks = (int)(gs_psnr_scratch_floats(batch, n) / batch);
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    k_sq_err_partial<<<dim3(blocks, batch), PS_THREADS, 0, st>>>(ground_truth, predicted, n, scratch);
-    GS_CUDA_OK(cudaGetLastError());
+    for (int64_t b0 = 0; b0 < batch; b0 += MAX_GRID_YZ) {
+        const int nb = (int)(batch - b0 < MAX_GRID_YZ ? batch - b0 : MAX_GRID_YZ);
+        k_sq_err_partial<<<dim3(blocks, nb), PS_THREADS, 0, st>>>(ground_truth + (size_t)b0 * n, predicted + (size_t)b0 * n, n,
+                                                                 scratch + (size_t)b0 * blocks);
+        GS_CUDA_OK(cudaGetLastError());
+    }
     k_psnr_finalize<<<batch, 32, 0, st>>>(scratch, blocks, n, out);
     GS_CUDA_OK(cudaGetLastError());
     return GS_OK;
@@ -178,7 +199,7 @@ extern "C" GS_API int64_t gs_ssim_scratch_floats(int32_t batch, int32_t channels
 
 extern "C" GS_API int gs_ssim(const float *ground_truth, const float *predicted, int32_t batch, int32_t channels,
                               int32_t height, int32_t width, float *scratch, float *out, void *stream) {
-    if (!ground_truth || !predicted || !scratch || !out || batch < 0 || channels < 1 || channels > 65535 || batch > 65535)
+    if (!ground_truth || !predicted || !scratch || !out || batch < 0 || channels < 1 || channels > MAX_GRID_YZ)
         return gs_set_error(GS_ERR_INVALID, "bad gs_ssim arguments");
     if (height < SS_TAPS || width < SS_TAPS)  // skimage: "win_size exceeds image extent"
         return gs_set_error(GS_ERR_INVALID, "gs_ssim: images must be at least 11 x 11 (win_size exceeds image extent)");
@@ -198,9 +219,13 @@ extern "C" GS_API int gs_ssim(const float *ground_truth, const float *predicted,
     const int tiles_x = (width - 2 * SS_R + SS_TILE - 1) / SS_TILE, tiles_y = (height - 2 * SS_R + SS_TILE - 1) / SS_TILE;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     double *partial = reinterpret_cast<double *>(scratch);
-    k_ssim_partial<<<dim3(tiles_x * tiles_y, channels, batch), SS_THREADS, 0, st>>>(ground_truth, predicted, height, width,
-                                                                                  tiles_x, tiles_y, wt, partial);
-    GS_CUDA_OK(cudaGetLastError());
+    const size_t image = (size_t)channels * height * width, per_image = (size_t)channels * tiles_x * tiles_y;
+    for (int64_t b0 = 0; b0 < batch; b0 += MAX_GRID_YZ) {
+        const int nb = (int)(batch - b0 < MAX_GRID_YZ ? batch - b0 : MAX_GRID_YZ);
+        k_ssim_partial<<<dim3(tiles_x * tiles_y, channels, nb), SS_THREADS, 0, st>>>(
+            ground_truth + b0 * image, predicted + b0 * image, height, width, tiles_x, tiles_y, wt, partial + b0 * per_image);
+        GS_CUDA_OK(cudaGetLastError());
+    }
     const double count = (double)channels * (double)(height - 2 * SS_R) * (double)(width - 2 * SS_R);
     k_ssim_finalize<<<batch, 32, 0, st>>>(partial, channels * tiles_x * tiles_y, count, out);
     GS_CUDA_OK(cudaGetLastError());

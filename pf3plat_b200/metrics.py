@@ -16,7 +16,9 @@ from .lpips import LPIPS
 
 @torch.no_grad()
 def compute_psnr(ground_truth: torch.Tensor, predicted: torch.Tensor) -> torch.Tensor:
-    """(batch, channel, height, width) x 2 -> (batch,) PSNR in dB; inputs are clipped to [0, 1]."""
+    """(batch, channel, height, width) x 2 -> (batch,) PSNR in dB; inputs are clipped to [0, 1] (a NaN stays NaN, so
+    an image holding one gets a NaN PSNR).  Computed in float32 and returned in torch.result_type(gt, pred), as the
+    reference's tensor arithmetic returns it."""
     if ground_truth.shape != predicted.shape or ground_truth.dim() < 2:
         raise ValueError("compute_psnr expects two tensors of the same (batch, ...) shape")
     if predicted.device.type != "cuda":
@@ -31,7 +33,7 @@ def compute_psnr(ground_truth: torch.Tensor, predicted: torch.Tensor) -> torch.T
         scratch = torch.empty((max(1, int(L.gs_psnr_scratch_floats(b, n))),), dtype=torch.float32, device=pr.device)
         _capi.check(L.gs_psnr(gt.data_ptr(), pr.data_ptr(), b, n, scratch.data_ptr(), out.data_ptr(),
                               torch.cuda.current_stream(pr.device).cuda_stream))
-    return out
+    return out.to(torch.result_type(ground_truth, predicted))
 
 
 @functools.cache

@@ -34,7 +34,7 @@
 extern "C" {
 #endif
 
-#define GS_ABI_VERSION 3
+#define GS_ABI_VERSION 4   /* 4: GsConfig::sh_eval_max_degree = 4 evaluates band 4 (3 clamped it to 3) */
 
 #if defined(__GNUC__)
 #define GS_API __attribute__((visibility("default")))
@@ -98,7 +98,11 @@ typedef struct GsConfig {
     float near_cull_z;    /* default 0.2 */
     float dilation;       /* default 0.3 */
     float guard_band;     /* default 1.3 */
-    int32_t sh_eval_max_degree; /* default 3 (<=0 selects it) */
+    /* Highest SH degree evaluated: default 3 (<=0 selects it), 4 opts in to band 4 (values above 4 evaluate 4).  The
+     * degree evaluated is min(sh_degree, sh_eval_max_degree, the largest degree M covers).  Degree 4 rejects
+     * GS_TUNE_PRE_OCC6 and GS_TUNE_PBWD_2PHASE (GS_ERR_INVALID).  ABI versions < 4 evaluated at most degree 3
+     * whatever this field said. */
+    int32_t sh_eval_max_degree;
     uint32_t tuning;      /* GS_TUNE_* implementation knobs (testing); 0 = default */
     const float *viewmatrix; /* device [V,16]  settings.viewmatrix */
     const float *projmatrix; /* device [V,16]  settings.projmatrix */

@@ -12,7 +12,7 @@ from ctypes import POINTER, Structure, c_char_p, c_float, c_int, c_int32, c_int6
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "csrc", "libgsplat_b200.so")
-ABI_VERSION = 3
+ABI_VERSION = 4
 
 GS_FLAG_DEPTH = 1
 GS_FLAG_PREFILTERED = 2

@@ -136,7 +136,7 @@ DevCfg make_dev_cfg(const GsConfig *cfg) {
     c.P = cfg->P; c.S = cfg->S; c.V = cfg->V; c.VPS = cfg->V / cfg->S; c.M = cfg->M;
     const int maxdeg = cfg->sh_eval_max_degree > 0 ? cfg->sh_eval_max_degree : 3;
     int deg = cfg->sh_degree < maxdeg ? cfg->sh_degree : maxdeg;
-    if (deg > 3) deg = 3;                                    // the evaluator implements bands 0..3
+    if (deg > 4) deg = 4;                                    // the evaluator implements bands 0..4
     while (deg > 0 && (deg + 1) * (deg + 1) > cfg->M) deg--;  // never read past the coefficients supplied
     if (deg < 0) deg = 0;
     c.deg = deg;

@@ -312,6 +312,20 @@ __device__ __forceinline__ float gs_rcp(float x) {
 #define GS_SH_C3_4 (-0.4570457994644658f)
 #define GS_SH_C3_5 1.445305721320277f
 #define GS_SH_C3_6 (-0.5900435899266435f)
+// band 4 (opt-in, GsConfig::sh_eval_max_degree = 4): the same real, orthonormal, Condon-Shortley-signed basis continued,
+// on the unit view direction.  Coefficients 16..24 multiply
+//   xy(xx-yy), yz(3xx-yy), xy(7zz-1), yz(7zz-3), zz(35zz-30)+3, xz(7zz-3), (xx-yy)(7zz-1), xz(xx-3yy),
+//   xx(xx-3yy)-yy(3xx-yy)
+// (the "-1" / "-3" forms hold on the unit sphere only; kernels and oracles use these forms alike)
+#define GS_SH_C4_0 2.5033429417967046f
+#define GS_SH_C4_1 (-1.7701307697799304f)
+#define GS_SH_C4_2 0.9461746957575601f
+#define GS_SH_C4_3 (-0.6690465435572892f)
+#define GS_SH_C4_4 0.10578554691520431f
+#define GS_SH_C4_5 (-0.6690465435572892f)
+#define GS_SH_C4_6 0.47308734787878004f
+#define GS_SH_C4_7 (-1.7701307697799304f)
+#define GS_SH_C4_8 0.6258357354491761f
 
 // ---- mbarrier + 1-D bulk TMA (cp.async.bulk) primitives ----
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }

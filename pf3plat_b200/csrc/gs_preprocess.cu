@@ -4,9 +4,10 @@
 // PF3plat's src/model/decoder/cuda_splatting.py:117-124).  Design (DESIGN.md section 5.1):
 //  * one thread per Gaussian, LOOPING over the views of its scene, so the scene-level inputs (mean, covariance
 //    and the 300-byte SH block) are read from HBM once per call instead of once per view;
-//  * the coefficients the evaluator reads (bands 0..3: 16 of PF3plat's 25) are staged into shared memory -- one 1-D
-//    bulk TMA copy (cp.async.bulk, SASS UBLKCP) completing on an mbarrier when M <= 16, a 4-byte cp.async gather into
-//    odd-stride rows otherwise -- fully coalesced, no register staging;
+//  * the coefficients the evaluator reads (bands 0..3 by default: 16 of PF3plat's 25; all 25 at the opt-in degree 4,
+//    the B4 instantiations) are staged into shared memory -- one 1-D bulk TMA copy (cp.async.bulk, SASS UBLKCP)
+//    completing on an mbarrier when they form a contiguous aligned block, a 4-byte cp.async gather into odd-stride
+//    rows otherwise -- fully coalesced, no register staging;
 //  * k_sh_colour (below): the colour words alone, pulled out of PINNED HOST memory, for gs_render_host's split pipeline,
 //    with k_preprocess running geometry-only (COLOUR = 0) next to it;
 //  * outputs are three float4 SoA planes written with 16-byte stores;
@@ -49,6 +50,8 @@ constexpr int PRE_SMEM_HDR = (sizeof(PreSmem) + 127) / 128 * 128;
 // left-to-right sum, +0.5, clamp at 0 with the clamp recorded per channel).  Every operation is an explicit
 // round-to-nearest intrinsic -- no contraction or re-association left to the compiler -- because TWO kernels inline this
 // function (k_preprocess and k_sh_colour, the split pipeline of gs_render_host) and must produce the same bits.
+// B4: band 4 is compiled in (evaluated when deg == 4); the default instantiation is the degree-<=3 evaluator unchanged.
+template <bool B4 = false>
 __device__ __forceinline__ float3 eval_sh(int deg, const float *sh /* [M][3] for this Gaussian */, float3 dir,
                                           uint32_t &clamped) {
     const float x = dir.x, y = dir.y, z = dir.z;
@@ -91,6 +94,28 @@ __device__ __forceinline__ float3 eval_sh(int deg, const float *sh /* [M][3] for
                     t = __fmaf_rn(b14, sh[14 * 3 + c], __fmaf_rn(b13, sh[13 * 3 + c], t));
                     v[c] = __fmaf_rn(b15, sh[15 * 3 + c], t);
                 }
+                if (B4 && deg > 3) {
+                    const float xx_yy = __fsub_rn(xx, yy), xx3_yy = __fsub_rn(__fmul_rn(3.0f, xx), yy);
+                    const float xx_3yy = __fsub_rn(xx, __fmul_rn(3.0f, yy)), zz7 = __fmul_rn(7.0f, zz);
+                    const float zz7m1 = __fsub_rn(zz7, 1.0f), zz7m3 = __fsub_rn(zz7, 3.0f);
+                    const float b16 = __fmul_rn(__fmul_rn(GS_SH_C4_0, xy), xx_yy);
+                    const float b17 = __fmul_rn(__fmul_rn(GS_SH_C4_1, yz), xx3_yy);
+                    const float b18 = __fmul_rn(__fmul_rn(GS_SH_C4_2, xy), zz7m1);
+                    const float b19 = __fmul_rn(__fmul_rn(GS_SH_C4_3, yz), zz7m3);
+                    const float b20 = __fmul_rn(GS_SH_C4_4, __fadd_rn(__fmul_rn(zz, __fsub_rn(__fmul_rn(35.0f, zz), 30.0f)), 3.0f));
+                    const float b21 = __fmul_rn(__fmul_rn(GS_SH_C4_5, xz), zz7m3);
+                    const float b22 = __fmul_rn(__fmul_rn(GS_SH_C4_6, xx_yy), zz7m1);
+                    const float b23 = __fmul_rn(__fmul_rn(GS_SH_C4_7, xz), xx_3yy);
+                    const float b24 = __fmul_rn(GS_SH_C4_8, __fsub_rn(__fmul_rn(xx, xx_3yy), __fmul_rn(yy, xx3_yy)));
+#pragma unroll
+                    for (int c = 0; c < 3; c++) {
+                        float t = __fmaf_rn(b17, sh[17 * 3 + c], __fmaf_rn(b16, sh[16 * 3 + c], v[c]));
+                        t = __fmaf_rn(b19, sh[19 * 3 + c], __fmaf_rn(b18, sh[18 * 3 + c], t));
+                        t = __fmaf_rn(b21, sh[21 * 3 + c], __fmaf_rn(b20, sh[20 * 3 + c], t));
+                        t = __fmaf_rn(b23, sh[23 * 3 + c], __fmaf_rn(b22, sh[22 * 3 + c], t));
+                        v[c] = __fmaf_rn(b24, sh[24 * 3 + c], t);
+                    }
+                }
             }
         }
     }
@@ -121,7 +146,7 @@ struct Splat {
 
 // Appendix A "Preprocess" for one Gaussian in one view.  COLOUR = 2: `sh` points at this Gaussian's [M][3] block in
 // shared memory; 1: `rgb_in` is its precomputed colour; 0: geometry only (the colour words are written by k_sh_colour).
-template <int COLOUR>
+template <int COLOUR, bool B4 = false>
 __device__ __forceinline__ void project_splat(const DevCfg &c, const ViewCam &cam, float3 mean, const float *c6,
                                               float opac, const float *sh, const float *rgb_in, Splat &out) {
     out.radius = 0;
@@ -160,7 +185,7 @@ __device__ __forceinline__ void project_splat(const DevCfg &c, const ViewCam &ca
     out.meta = GS_META_VISIBLE;
     float3 rgb;
     if (COLOUR == 2 && (ABL & ABL_SH)) rgb = make_float3(0.5f, 0.5f, 0.5f);
-    else if (COLOUR == 2) rgb = eval_sh(c.deg, sh, sh_view_dir(m, cam.campos), out.meta);
+    else if (COLOUR == 2) rgb = eval_sh<B4>(c.deg, sh, sh_view_dir(m, cam.campos), out.meta);
     else if (COLOUR == 1) rgb = make_float3(rgb_in[0], rgb_in[1], rgb_in[2]);
     else rgb = make_float3(0.f, 0.f, 0.f);   // COLOUR == 0: k_sh_colour fills the three colour words of the record
     // Tight binning.  A pixel can only receive this Gaussian if alpha = o*G >= 1/255, i.e. log2 G >= -log2(255 o).
@@ -182,7 +207,8 @@ __device__ __forceinline__ void project_splat(const DevCfg &c, const ViewCam &ca
 
 // MINB: resident CTAs per SM the register allocation is bounded for.  Unbounded the kernel takes 96 registers (5 CTAs/SM;
 // latency-bound).  Bounded to 64 (8 CTAs/SM, 116 bytes of spills and more instructions) it was slower on C2.
-template <int COLOUR, int MINB>
+// B4: degree-4 evaluation (25 coefficients staged per Gaussian); the B4 = false kernels are the degree-<=3 ones unchanged.
+template <int COLOUR, int MINB, bool B4 = false>
 __global__ void __launch_bounds__(PRE_THREADS, MINB)
 k_preprocess(const DevCfg c, const DevInputs in, float4 *__restrict__ rec0, float4 *__restrict__ rec1,
              float4 *__restrict__ rec2, uint8_t *__restrict__ meta, int32_t *__restrict__ radii,
@@ -213,8 +239,12 @@ k_preprocess(const DevCfg c, const DevInputs in, float4 *__restrict__ rec0, floa
     //    cp.async, SASS LDGSTS.128).  Built for a source in PINNED HOST memory, which is pulled over PCIe faster by
     //    16-byte loads than by 4-byte ones (scripts/probes/pcie_pull_probe.cu compares them with the copy engine).  On
     //    device-resident SH it loses to the compacting gather (38 instead of 25 KB of shared memory per CTA leave the L1 28 KB at five CTAs per SM).
-    const int MS = c.M < 16 ? c.M : 16;
-    const int RS = (c.M == MS || sh_raw16) ? c.M * 3 : 49;   // floats per staged row (3 M = 75 for PF3plat: 11 t mod 32, conflict-free)
+    //  * B4 (degree 4): all 25 coefficients are wanted, so for PF3plat's M = 25 the block is contiguous again: one bulk TMA
+    //    copy when it is 16-byte aligned, else a 4-byte cp.async gather; rows keep their own odd stride of 75 floats.
+    //    (M > 25 compacts to 75 floats.)  The B4 constants are spelled inline: named constexpr locals, though folded
+    //    away, renumber the front end's virtual registers and perturb the default kernels' register allocation.
+    const int MS = c.M < (B4 ? 25 : 16) ? c.M : (B4 ? 25 : 16);
+    const int RS = (c.M == MS || sh_raw16) ? c.M * 3 : (B4 ? 75 : 49);   // floats per staged row (3 M = 75 for PF3plat: 11 t mod 32, conflict-free)
     constexpr bool HAS_SH = COLOUR == 2;
     bool bulk = false;
     if (HAS_SH && !(ABL & ABL_SH)) {
@@ -229,6 +259,9 @@ k_preprocess(const DevCfg c, const DevInputs in, float4 *__restrict__ rec0, floa
                     mbar_expect_tx(&sm->bar, bytes);
                     tma_load_1d(sh_s, src, bytes, &sm->bar);
                 }
+            } else if constexpr (B4) {  // unaligned slice or ragged tail: asynchronous coalesced 4-byte copies
+                for (uint32_t k = tid; k < (uint32_t)n * c.M * 3u; k += PRE_THREADS) cp_async4(sh_s + k, src + k);
+                cp_async_commit();
             } else {  // unaligned slice or ragged tail: plain coalesced copy
                 for (uint32_t k = tid; k < (uint32_t)n * c.M * 3u; k += PRE_THREADS) sh_s[k] = src[k];
             }
@@ -247,9 +280,9 @@ k_preprocess(const DevCfg c, const DevInputs in, float4 *__restrict__ rec0, floa
             // asynchronous 4-byte copies (cp.async, SASS LDGSTS): all 48 per thread are in flight together while the
             // scalar inputs load -- a plain load/store loop here serialises the latencies
             const uint32_t row_f = (uint32_t)c.M * 3u;
-            for (uint32_t e = tid; e < (uint32_t)n * 48u; e += PRE_THREADS) {
-                const uint32_t row = e / 48u, col = e - row * 48u;
-                cp_async4(sh_s + row * 49u + col, src + (size_t)row * row_f + col);
+            for (uint32_t e = tid; e < (uint32_t)n * (B4 ? 75u : 48u); e += PRE_THREADS) {
+                const uint32_t row = e / (B4 ? 75u : 48u), col = e - row * (B4 ? 75u : 48u);
+                cp_async4(sh_s + row * (B4 ? 75u : 49u) + col, src + (size_t)row * row_f + col);
             }
             cp_async_commit();
         }
@@ -319,7 +352,7 @@ k_preprocess(const DevCfg c, const DevInputs in, float4 *__restrict__ rec0, floa
             const int v = scene * c.VPS + v0 + vi;
             const size_t o = (size_t)v * c.P + i;
             Splat sp;
-            project_splat<COLOUR>(c, sm->cams[vi], mean, c6, opac, sh_s + (size_t)tid * RS,
+            project_splat<COLOUR, B4>(c, sm->cams[vi], mean, c6, opac, sh_s + (size_t)tid * RS,
                                   COLOUR == 1 ? in.colors_precomp + o * 3 : nullptr, sp);
             // fused speculative emission: nothing reads the rects afterwards (k_emit_buckets and the strata learning, their
             // readers, run on the other paths only)
@@ -436,6 +469,7 @@ k_preprocess(const DevCfg c, const DevInputs in, float4 *__restrict__ rec0, floa
 constexpr int SHC_THREADS = 128;
 constexpr int SHC_VIEWS = 64;   // cameras staged at a time
 
+template <bool B4 = false>   // B4: degree 4, all 25 coefficients of a row are pulled
 __global__ void __launch_bounds__(SHC_THREADS, 3)
 k_sh_colour(const DevCfg c, const float *__restrict__ means3D, const float *__restrict__ shs, float4 *__restrict__ rec1,
             float4 *__restrict__ rec2, uint8_t *__restrict__ clamp_out /* [V*P] or NULL */, const int blocks_per_scene) {
@@ -443,7 +477,8 @@ k_sh_colour(const DevCfg c, const float *__restrict__ means3D, const float *__re
     float4 *cam_s = reinterpret_cast<float4 *>(smem_raw);                    // (campos xyz, scale) per staged view
     float *sh_s = reinterpret_cast<float *>(smem_raw + SHC_VIEWS * sizeof(float4));
     const int tid = threadIdx.x;
-    const uint32_t row_f = (uint32_t)c.M * 3u, want_f = (uint32_t)(c.M < 16 ? c.M : 16) * 3u;
+    constexpr int MSMAX = B4 ? 25 : 16;
+    const uint32_t row_f = (uint32_t)c.M * 3u, want_f = (uint32_t)(c.M < MSMAX ? c.M : MSMAX) * 3u;
     const int total = blocks_per_scene * c.S;
     for (int blk = blockIdx.x; blk < total; blk += gridDim.x) {
         const int scene = blk / blocks_per_scene, g0 = (blk - scene * blocks_per_scene) * SHC_THREADS;
@@ -482,7 +517,7 @@ k_sh_colour(const DevCfg c, const float *__restrict__ means3D, const float *__re
                 const float3 m = make_float3(mean.x * cam.w, mean.y * cam.w, mean.z * cam.w);
                 const float cp[3] = {cam.x, cam.y, cam.z};
                 uint32_t clamped = 0;
-                const float3 rgb = eval_sh(c.deg, sh, sh_view_dir(m, cp), clamped);
+                const float3 rgb = eval_sh<B4>(c.deg, sh, sh_view_dir(m, cp), clamped);
                 reinterpret_cast<float2 *>(&rec1[o])[1] = make_float2(rgb.x, rgb.y);
                 reinterpret_cast<float *>(&rec2[o])[0] = rgb.z;
                 if (clamp_out) clamp_out[o] = (uint8_t)clamped;
@@ -520,7 +555,12 @@ int launch_preprocess(const DevCfg &c, const DevInputs &in, float4 *rec0, float4
         const uintptr_t first = reinterpret_cast<uintptr_t>(in.shs) + (size_t)g_begin * c.M * 12;
         sh_raw16 = (first & 15u) == 0 && (c.S == 1 || ((size_t)c.P * c.M * 12) % 16 == 0);
     }
-    const size_t smem = PRE_SMEM_HDR + ((in.shs && !(variant & 4)) ? (size_t)PRE_THREADS * ((c.M <= 16 || sh_raw16) ? c.M * 3 : 49) * 4 : 0);
+    // degree 4 evaluates (and stages) 25 coefficients per Gaussian: the B4 kernel
+    const bool b4 = in.shs && !(variant & 4) && c.deg > 3;
+    if (b4 && more_ctas)
+        return gs_set_error(GS_ERR_INVALID, "GS_TUNE_PRE_OCC6 has no degree-4 kernel (sh_eval_max_degree = 4)");
+    const int max_rs = b4 ? 75 : 49;   // floats per compacted row
+    const size_t smem = PRE_SMEM_HDR + ((in.shs && !(variant & 4)) ? (size_t)PRE_THREADS * ((c.M <= (b4 ? 25 : 16) || sh_raw16) ? c.M * 3 : max_rs) * 4 : 0);
     if (smem > (size_t)227 * 1024) return gs_set_error(GS_ERR_INVALID, "too many SH coefficients per Gaussian for the staging buffer");
     auto launch = [&](auto kern) -> int {
         GS_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -529,6 +569,7 @@ int launch_preprocess(const DevCfg &c, const DevInputs &in, float4 *rec0, float4
     };
     int rc;
     if (variant & 4) rc = more_ctas ? launch(k_preprocess<0, 6>) : launch(k_preprocess<0, 5>);   // geometry only
+    else if (b4) rc = launch(k_preprocess<2, 5, true>);
     else if (in.shs) rc = more_ctas ? launch(k_preprocess<2, 6>) : launch(k_preprocess<2, 5>);
     else rc = more_ctas ? launch(k_preprocess<1, 6>) : launch(k_preprocess<1, 5>);
     if (rc != GS_OK) return rc;
@@ -561,8 +602,9 @@ int launch_sh_colour(const DevCfg &c, const DevInputs &in, float4 *rec1, float4 
     const int per_sm = 3;
     const int grid = (int)(total < (long long)sms * per_sm ? total : (long long)sms * per_sm);
     const size_t smem = SHC_VIEWS * sizeof(float4) + (size_t)SHC_THREADS * c.M * 12;
-    GS_CUDA_OK(cudaFuncSetAttribute(k_sh_colour, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    k_sh_colour<<<grid, SHC_THREADS, smem, st>>>(c, in.means3D, in.shs, rec1, rec2, clamp_out, bps);
+    auto kern = c.deg > 3 ? k_sh_colour<true> : k_sh_colour<false>;
+    GS_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    kern<<<grid, SHC_THREADS, smem, st>>>(c, in.means3D, in.shs, rec1, rec2, clamp_out, bps);
     GS_CUDA_OK(cudaGetLastError());
     return GS_OK;
 }

@@ -26,6 +26,7 @@ struct PbSmem {
 constexpr int PB_SMEM_HDR = (sizeof(PbSmem) + 127) / 128 * 128;
 
 constexpr int PB_SH_EVAL = 16;  // coefficients per channel the evaluator can touch (bands 0..3)
+constexpr int PB_SH_B4 = 27;    // band-4 accumulators per Gaussian (9 coefficients x 3 channels), degree-4 kernels only
 
 // dL/dsh_k += basis_k(dir) * g  and  dL/ddir, for one colour channel.  sh: stride-3 view of this channel's
 // coefficients in shared memory; gsh: stride-3 view of this channel's accumulators (REGISTERS: all indices are
@@ -75,6 +76,47 @@ __device__ __forceinline__ void sh_backward_channel(int deg, const float *sh, fl
     ddx += dx_ * g;
     ddy += dy_ * g;
     ddz += dz_ * g;
+}
+
+// Band 4 (degree-4 kernels only): dL/dsh_k += basis_k(dir) * g_ch for k = 16..24 and all three channels, and band 4's
+// share of dL/ddir.  sh: this Gaussian's staged [M][3] row; g4: its [9][3] band-4 accumulators in SHARED memory (see
+// k_preprocess_bwd).  Same polynomial forms as eval_sh (gs_preprocess.cu); their partial derivatives in x, y, z taken as
+// independent variables (the "-1" / "-3" forms differ from homogeneous ones only along dir, which the normalisation
+// projects out).
+__device__ __forceinline__ void sh_backward_band4(const float *sh, float *g4, const float g[3], float x, float y, float z,
+                                                  float &ddx, float &ddy, float &ddz) {
+    const float xx = x * x, yy = y * y, zz = z * z, xy = x * y, yz = y * z, xz = x * z;
+    const float xx_yy = xx - yy, xx3_yy = 3.0f * xx - yy, xx_3yy = xx - 3.0f * yy;
+    const float zz7m1 = 7.0f * zz - 1.0f, zz7m3 = 7.0f * zz - 3.0f, zz21m3 = 21.0f * zz - 3.0f;
+    // basis value and its partials (d/dx, d/dy, d/dz) per coefficient 16 + k
+    const float B[9] = {GS_SH_C4_0 * xy * xx_yy, GS_SH_C4_1 * yz * xx3_yy, GS_SH_C4_2 * xy * zz7m1,
+                        GS_SH_C4_3 * yz * zz7m3, GS_SH_C4_4 * (zz * (35.0f * zz - 30.0f) + 3.0f), GS_SH_C4_5 * xz * zz7m3,
+                        GS_SH_C4_6 * xx_yy * zz7m1, GS_SH_C4_7 * xz * xx_3yy,
+                        GS_SH_C4_8 * (xx * xx_3yy - yy * xx3_yy)};
+    const float DX[9] = {GS_SH_C4_0 * y * xx3_yy, GS_SH_C4_1 * 6.0f * x * yz, GS_SH_C4_2 * y * zz7m1, 0.0f, 0.0f,
+                         GS_SH_C4_5 * z * zz7m3, GS_SH_C4_6 * 2.0f * x * zz7m1, GS_SH_C4_7 * 3.0f * z * xx_yy,
+                         GS_SH_C4_8 * 4.0f * x * xx_3yy};
+    const float DY[9] = {GS_SH_C4_0 * x * xx_3yy, GS_SH_C4_1 * 3.0f * z * xx_yy, GS_SH_C4_2 * x * zz7m1,
+                         GS_SH_C4_3 * z * zz7m3, 0.0f, 0.0f, GS_SH_C4_6 * -2.0f * y * zz7m1, GS_SH_C4_7 * -6.0f * x * yz,
+                         GS_SH_C4_8 * -4.0f * y * xx3_yy};
+    const float DZ[9] = {0.0f, GS_SH_C4_1 * y * xx3_yy, GS_SH_C4_2 * 14.0f * xy * z, GS_SH_C4_3 * y * zz21m3,
+                         GS_SH_C4_4 * z * (140.0f * zz - 60.0f), GS_SH_C4_5 * x * zz21m3, GS_SH_C4_6 * 14.0f * z * xx_yy,
+                         GS_SH_C4_7 * x * xx_3yy, 0.0f};
+    float dx_ = 0.f, dy_ = 0.f, dz_ = 0.f;
+#pragma unroll
+    for (int k = 0; k < 9; k++) {
+#pragma unroll
+        for (int ch = 0; ch < 3; ch++) {
+            g4[k * 3 + ch] += B[k] * g[ch];
+            const float w = sh[(16 + k) * 3 + ch] * g[ch];
+            dx_ += DX[k] * w;
+            dy_ += DY[k] * w;
+            dz_ += DZ[k] * w;
+        }
+    }
+    ddx += dx_;
+    ddy += dy_;
+    ddz += dz_;
 }
 
 // dL/d(view matrix entries 2, 6, 10, 14) of one view += the warp's sum of (gz * m, gz): a butterfly over the 32 lanes,
@@ -132,13 +174,22 @@ __device__ __forceinline__ const float *load_det_acc(const DetAcc &det, size_t o
 // (z = view[2] m.x + view[6] m.y + view[10] m.z + view[14], m the view-scaled mean).  The default instantiations
 // (VIEW_Z = false) are the kernels without it, instruction for instruction.  DET: the accumulators are the fixed-point
 // ones of the deterministic backward (det.acc, det.poison) and the view-matrix gradient goes through det.view_z.
-template <bool HAS_SH, int MINB, bool VIEW_Z = false, bool DET = false>
+// B4: degree 4 (c.deg == 4, M >= 25).  The 48 accumulators of bands 0..3 stay in registers as in the default kernel; the
+// 27 of band 4 live in a shared-memory row per thread next to the staged inputs (stride 27, odd: conflict-free), which
+// keeps the register bound -- and so the 4 resident CTAs per SM -- of the default kernel.
+template <bool HAS_SH, int MINB, bool VIEW_Z = false, bool DET = false, bool B4 = false>
 __global__ void __launch_bounds__(PB_THREADS, MINB)
 k_preprocess_bwd(const DevCfg c, const DevInputs in, const uint8_t *__restrict__ meta, const float *__restrict__ acc,
                     const GsInGrads g, const DetAcc det) {
     extern __shared__ __align__(128) unsigned char smem_raw[];
     PbSmem *sm = reinterpret_cast<PbSmem *>(smem_raw);
     float *sh_s = reinterpret_cast<float *>(smem_raw + PB_SMEM_HDR);
+    // B4: this thread's band-4 accumulators, behind the staged block of PB_THREADS rows
+    float *g4 = B4 ? sh_s + (size_t)PB_THREADS * c.M * 3 + (size_t)threadIdx.x * PB_SH_B4 : nullptr;
+    if constexpr (B4) {
+#pragma unroll
+        for (int k = 0; k < PB_SH_B4; k++) g4[k] = 0.f;
+    }
 
     const int scene = blockIdx.y;
     const int g0 = blockIdx.x * PB_THREADS;
@@ -297,6 +348,10 @@ k_preprocess_bwd(const DevCfg c, const DevInputs in, const uint8_t *__restrict__
                     const float gch = (mb & (1u << ch)) ? 0.0f : gcol[ch];
                     sh_backward_channel(c.deg, sh + ch, gsh + ch, gch, x, y, z, ddx, ddy, ddz);
                 }
+                if constexpr (B4) {
+                    const float g3[3] = {(mb & 1u) ? 0.0f : gcol[0], (mb & 2u) ? 0.0f : gcol[1], (mb & 4u) ? 0.0f : gcol[2]};
+                    sh_backward_band4(sh, g4, g3, x, y, z, ddx, ddy, ddz);
+                }
                 const float dot = d[0] * ddx + d[1] * ddy + d[2] * ddz;
                 const float inv3 = inv * inv * inv;
                 gm[0] += (ddx * len2 - d[0] * dot) * inv3;
@@ -374,7 +429,13 @@ k_preprocess_bwd(const DevCfg c, const DevInputs in, const uint8_t *__restrict__
 #pragma unroll
             for (int k = 0; k < PB_SH_EVAL * 3; k++)
                 if (k < used) row[k] = gsh[k];
-            for (int k = used; k < c.M * 3; k++) row[k] = 0.f;
+            if constexpr (B4) {   // M >= 25: band 4 follows from the shared accumulators, zeros beyond it
+#pragma unroll
+                for (int k = 0; k < PB_SH_B4; k++) row[PB_SH_EVAL * 3 + k] = g4[k];
+                for (int k = PB_SH_EVAL * 3 + PB_SH_B4; k < c.M * 3; k++) row[k] = 0.f;
+            } else {
+                for (int k = used; k < c.M * 3; k++) row[k] = 0.f;
+            }
         }
         if (bulk) {
             fence_proxy_async_smem();  // make the generic-proxy smem writes visible to the TMA engine
@@ -700,7 +761,14 @@ template <bool VIEW_Z, bool DET>
 int launch_preprocess_bwd_t(const DevCfg &c, const DevInputs &in, const GsSaved &s, const float *grad_acc,
                             const GsInGrads &g, cudaStream_t st, int variant, const DetAcc &det) {
     dim3 grid((c.P + PB_THREADS - 1) / PB_THREADS, c.S);
-    if (variant != 1) {  // single pass over the views (default)
+    if (in.shs && c.deg > 3) {   // degree 4: the single-pass kernel with band 4 compiled in
+        if (variant == 1)
+            return gs_set_error(GS_ERR_INVALID, "GS_TUNE_PBWD_2PHASE has no degree-4 kernel (sh_eval_max_degree = 4)");
+        const size_t smem = PB_SMEM_HDR + (size_t)PB_THREADS * (c.M * 3 + PB_SH_B4) * 4;
+        auto kern = k_preprocess_bwd<true, PB_MIN_CTAS, VIEW_Z, DET, true>;
+        GS_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        kern<<<grid, PB_THREADS, smem, st>>>(c, in, s.meta, grad_acc, g, det);
+    } else if (variant != 1) {  // single pass over the views (default)
         if (in.shs) {
             size_t smem = PB_SMEM_HDR + (size_t)PB_THREADS * c.M * 12;
             GS_CUDA_OK(cudaFuncSetAttribute(k_preprocess_bwd<true, PB_MIN_CTAS, VIEW_Z, DET>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));

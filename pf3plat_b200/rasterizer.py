@@ -165,6 +165,43 @@ class BatchSettings(NamedTuple):
     with_depth: bool = False
     debug: bool = False
     tuning: int = 0                          # GS_TUNE_* knobs (testing)
+    # highest SH degree evaluated (GsConfig.sh_eval_max_degree): 3, or 4 to evaluate and train band 4 of a 25-coefficient
+    # block; None = the process-wide setting (set_sh_eval_max_degree)
+    sh_eval_max_degree: Optional[int] = None
+
+
+# ---------------------------------------------------------------------------------------------------------
+# highest SH degree evaluated, for callers that cannot pass BatchSettings (the drop-in GaussianRasterizer)
+# ---------------------------------------------------------------------------------------------------------
+_sh_eval_max_degree = 3
+
+
+def set_sh_eval_max_degree(degree: int) -> None:
+    """Process-wide highest SH degree the rasterizer evaluates when BatchSettings.sh_eval_max_degree is None: 3 (the
+    default: bands 0..3, as upstream) or 4 (band 4 too, for 25-coefficient blocks such as PF3plat's adapter output).
+    The degree evaluated is min(sh_degree, this, the largest degree the coefficients cover).  A forward's backward uses
+    the degree that forward used, whatever the setting is by then."""
+    global _sh_eval_max_degree
+    _sh_eval_max_degree = _check_degree(degree)
+
+
+def get_sh_eval_max_degree() -> int:
+    return _sh_eval_max_degree
+
+
+def _check_degree(degree) -> int:
+    # (GsConfig.sh_eval_max_degree <= 0 selects the library default 3, so 0 cannot be expressed; sh_degree = 0 can)
+    degree = int(degree)
+    if degree < 1:
+        raise ValueError(f"sh_eval_max_degree must be >= 1, got {degree}")
+    return degree
+
+
+def _resolve_degree(bs: BatchSettings) -> BatchSettings:
+    """bs with sh_eval_max_degree made explicit (the process-wide setting in place of None)."""
+    if bs.sh_eval_max_degree is None:
+        return bs._replace(sh_eval_max_degree=_sh_eval_max_degree)
+    return bs
 
 
 def _make_config(bs: BatchSettings, S: int, P: int, M: int, keep: list) -> GsConfig:
@@ -178,6 +215,7 @@ def _make_config(bs: BatchSettings, S: int, P: int, M: int, keep: list) -> GsCon
     cfg.tanfovx, cfg.tanfovy = float(bs.tanfovx), float(bs.tanfovy)
     cfg.scale_modifier = float(bs.scale_modifier)
     cfg.tuning = int(bs.tuning)
+    cfg.sh_eval_max_degree = _check_degree(_sh_eval_max_degree if bs.sh_eval_max_degree is None else bs.sh_eval_max_degree)
     tensors = {
         "viewmatrix": _f32c(bs.viewmatrix).reshape(V, 16), "projmatrix": _f32c(bs.projmatrix, dev).reshape(V, 16),
         "campos": _f32c(bs.campos, dev).reshape(V, 3), "bg": _f32c(bs.bg, dev).reshape(V, 3),
@@ -205,6 +243,8 @@ class _RasterizeBatch(torch.autograd.Function):
         # an output the loss does not use arrives in backward as None instead of a zero tensor: a colour-only loss
         # then gives the view matrices no gradient at all (and the kernels read no depth gradient: the same sums)
         ctx.set_materialize_grads(False)
+        # the SH degree this forward evaluates is fixed here: ctx.bs carries it to the backward
+        bs = _resolve_degree(bs)
         dev = means3D.device
         if dev.type != "cuda":
             raise RuntimeError("pf3plat_b200 rasterizer needs CUDA tensors (there is no CPU fallback)")

@@ -32,10 +32,13 @@ def _cov6(cov: torch.Tensor) -> torch.Tensor:
 
 def render_views(extrinsics, intrinsics, near, far, image_shape, background_color, gaussian_means,
                  gaussian_covariances, gaussian_sh_coefficients, gaussian_opacities, scale_invariant: bool = True,
-                 use_sh: bool = True, with_depth: bool = False, sh_layout: str = "g_xyz_n"):
+                 use_sh: bool = True, with_depth: bool = False, sh_layout: str = "g_xyz_n",
+                 sh_eval_max_degree: Optional[int] = None):
     """extrinsics (B,4,4) c2w, intrinsics (B,3,3), near/far (B,), background (B,3); Gaussians are per SCENE and NOT
     repeated per view: means (S,G,3), covariances (S,G,3,3) or (S,G,6), sh (S,G,3,d_sh) [or (S,G,d_sh,3) with
     sh_layout="g_n_xyz"], opacities (S,G); B % S == 0 and view b shows scene b // (B//S).
+    sh_eval_max_degree: highest SH degree evaluated (3, or 4 for band 4 of d_sh = 25); None = the process-wide setting
+    (rasterizer.set_sh_eval_max_degree, default 3).
     Returns color (B,3,h,w) and, if with_depth, depth (B,h,w) = sum_i alpha_i T_i z_i."""
     assert use_sh or gaussian_sh_coefficients.shape[-1 if sh_layout == "g_xyz_n" else -2] == 1
     h, w = image_shape
@@ -51,7 +54,8 @@ def render_views(extrinsics, intrinsics, near, far, image_shape, background_colo
         else _cov6(gaussian_covariances)
     bs = BatchSettings(image_height=h, image_width=w, viewmatrix=vb.viewmatrix, projmatrix=vb.projmatrix,
                        campos=vb.campos, bg=background_color, sh_degree=degree, tanfov=vb.tanfov,
-                       view_scale=vb.scale if scale_invariant else None, with_depth=with_depth)
+                       view_scale=vb.scale if scale_invariant else None, with_depth=with_depth,
+                       sh_eval_max_degree=sh_eval_max_degree)
     B = extrinsics.shape[0]
     S = gaussian_means.shape[0]
     if use_sh:
@@ -74,7 +78,7 @@ def render_cuda(extrinsics, intrinsics, near, far, image_shape, background_color
 
 
 def decoder_forward(means, covariances, harmonics, opacities, extrinsics, intrinsics, near, far, image_shape,
-                    background_color, depth_mode: Optional[str] = None):
+                    background_color, depth_mode: Optional[str] = None, sh_eval_max_degree: Optional[int] = None):
     """`DecoderSplattingCUDA.forward` (decoder_splatting_cuda.py:35-67) without the v-fold repeat: Gaussians
     (b,g,...), cameras (b,v,...).  Returns (color (b,v,3,h,w), depth (b,v,h,w) or None).  depth_mode "depth" is
     fused into the colour pass; the reference's other modes are served by `render_depth`.
@@ -85,13 +89,14 @@ def decoder_forward(means, covariances, harmonics, opacities, extrinsics, intrin
     channel gives exactly that gradient and no other: dL/ddepth reaches the z column of each view matrix
     (make_view_batch carries it on to the extrinsics), besides the Gaussians.  A loss that does not read the depth
     leaves the extrinsics without a gradient, as the reference does.  So "depth" is one render whether or not the
-    extrinsics require grad."""
+    extrinsics require grad.  sh_eval_max_degree: as render_views."""
     b, v = extrinsics.shape[:2]
     flat = lambda t: t.reshape(b * v, *t.shape[2:])
     bg = background_color.reshape(1, 3).expand(b * v, 3)
     if depth_mode is None or depth_mode == "depth":
         out = render_views(flat(extrinsics), flat(intrinsics), flat(near), flat(far), image_shape, bg, means,
-                           covariances, harmonics, opacities, with_depth=depth_mode is not None)
+                           covariances, harmonics, opacities, with_depth=depth_mode is not None,
+                           sh_eval_max_degree=sh_eval_max_degree)
         if depth_mode is None:
             return out.reshape(b, v, *out.shape[1:]), None
         color, depth = out
@@ -101,7 +106,7 @@ def decoder_forward(means, covariances, harmonics, opacities, extrinsics, intrin
         depth = depth * flat(near)[:, None, None]
         return color.reshape(b, v, *color.shape[1:]), depth.reshape(b, v, *depth.shape[1:])
     color = render_views(flat(extrinsics), flat(intrinsics), flat(near), flat(far), image_shape, bg, means,
-                         covariances, harmonics, opacities)
+                         covariances, harmonics, opacities, sh_eval_max_degree=sh_eval_max_degree)
     depth = render_depth(means, covariances, opacities, extrinsics, intrinsics, near, far, image_shape, depth_mode)
     return color.reshape(b, v, *color.shape[1:]), depth
 

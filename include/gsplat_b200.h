@@ -34,7 +34,7 @@
 extern "C" {
 #endif
 
-#define GS_ABI_VERSION 4   /* 4: GsConfig::sh_eval_max_degree = 4 evaluates band 4 (3 clamped it to 3) */
+#define GS_ABI_VERSION 5   /* 5: GsConfig::depth_mode, depth_near_far appended; 4: sh_eval_max_degree = 4 evaluates band 4 */
 
 #if defined(__GNUC__)
 #define GS_API __attribute__((visibility("default")))
@@ -52,7 +52,7 @@ enum {
 };
 
 enum {
-    GS_FLAG_DEPTH = 1u,        /* also composite camera-space z as a 4th channel (render_depth_cuda mode "depth", cuda_splatting.py:226-269, fused) */
+    GS_FLAG_DEPTH = 1u,        /* also composite a depth channel (render_depth_cuda, cuda_splatting.py:226-269, fused): camera-space z, or f(z) of GsConfig::depth_mode */
     GS_FLAG_PREFILTERED = 2u,  /* GaussianRasterizationSettings.prefiltered */
     /* gs_backward: bit-reproducible gradients.  The composite backward adds its per-(view, Gaussian) terms as exact
      * fixed-point integers (2^-80 resolution, terms up to 2^45 in magnitude; NaN, Inf or larger terms make that gradient
@@ -79,6 +79,16 @@ enum {
     GS_TUNE_NO_ZERO_COPY = 131072u,   /* gs_render_host: always upload the SH block with the copy engine (in pieces) even when the caller's buffer is pinned and preprocess could pull it over PCIe itself (A/B) */
     GS_TUNE_NO_SPLIT_COLOUR = 262144u, /* gs_render_host, zero-copy feed: one fused preprocess pulling the SH block instead of geometry + tile sort on the launch stream with k_sh_colour pulling the block on a second stream (A/B) */
     GS_TUNE_FEED_PIECES_SHIFT = 8     /* gs_render_host: bits 8..11 = pieces the SH block is copied in (0 default, 1 = one plain copy) */
+};
+
+/* What the depth channel (GS_FLAG_DEPTH) composites: PF3plat's DepthRenderingMode (cuda_splatting.py:223-251), whose
+ * fake colour f(z) render_depth_cuda builds from the UNSCALED camera-space depth z of each mean and the unscaled near
+ * and far of the view.  The kernels see z_s = view_scale * z and evaluate f at z = z_s / view_scale. */
+enum {
+    GS_DEPTH_Z = 0,                  /* "depth": z_s itself (the caller multiplies by 1 / view_scale); default */
+    GS_DEPTH_DISPARITY = 1,          /* "disparity": 1 / z */
+    GS_DEPTH_RELATIVE_DISPARITY = 2, /* "relative_disparity": 1 - (1/(z+e) - 1/(far+e)) / (1/(near+e) - 1/(far+e) + e), e = 1e-10 */
+    GS_DEPTH_LOG = 3                 /* "log": log(max(min(z, near), far)) -- the reference's clamp as written: log(far) for near < far */
 };
 
 /* GaussianRasterizationSettings (cuda_splatting.py:99-112), batched over views. */
@@ -111,6 +121,11 @@ typedef struct GsConfig {
     const float *tanfov;     /* device [V,2] or NULL */
     const float *view_scale; /* device [V] or NULL: per-view factor s applied as mean*s, cov*s^2, scales*s
                                 (the 1/near rescale of cuda_splatting.py:64-71 without materialising copies) */
+    /* GS_DEPTH_*: what the depth channel composites.  A mode other than GS_DEPTH_Z needs GS_FLAG_DEPTH; an unknown mode,
+     * or GS_DEPTH_RELATIVE_DISPARITY / GS_DEPTH_LOG without depth_near_far, is GS_ERR_INVALID.  A backward uses the mode
+     * of its forward (the field is ignored there, depth_near_far is read again).  dL_dviewmatrix_z works in every mode. */
+    int32_t depth_mode;
+    const float *depth_near_far; /* device [V,2]: unscaled (near, far) per view, or NULL (GS_DEPTH_Z, GS_DEPTH_DISPARITY) */
 } GsConfig;
 
 /* Arguments of GaussianRasterizer.forward (cuda_splatting.py:117-124).  Exactly one of shs/colors_precomp and
@@ -151,7 +166,8 @@ typedef struct GsInGrads {
     float *dL_dcov3D;      /* device [S,P,6] */
     /* device [V,4]: dL/d(viewmatrix flat entries 2, 6, 10, 14), the z column of the transposed view matrix, through the
      * fused depth channel only (z = that column . (view_scale * mean, 1)), as render_depth_cuda's fake colour carries it
-     * (cuda_splatting.py:239-242).  Colour, projection and culling give the cameras no gradient.  NULL = not wanted;
+     * (cuda_splatting.py:239-242); in a depth mode other than GS_DEPTH_Z, through f(z) of that mode (GS_DEPTH_LOG with
+     * near < far: zeros).  Colour, projection and culling give the cameras no gradient.  NULL = not wanted;
      * needs GS_FLAG_DEPTH.  Written, not accumulated; zeros when dL_ddepth is NULL. */
     float *dL_dviewmatrix_z;
 } GsInGrads;

@@ -12,11 +12,18 @@ from ctypes import POINTER, Structure, c_char_p, c_float, c_int, c_int32, c_int6
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "csrc", "libgsplat_b200.so")
-ABI_VERSION = 4
+ABI_VERSION = 5
 
 GS_FLAG_DEPTH = 1
 GS_FLAG_PREFILTERED = 2
 GS_FLAG_DETERMINISTIC = 4
+GS_DEPTH_Z = 0
+GS_DEPTH_DISPARITY = 1
+GS_DEPTH_RELATIVE_DISPARITY = 2
+GS_DEPTH_LOG = 3
+# PF3plat's DepthRenderingMode names -> GsConfig.depth_mode
+DEPTH_MODES = {"depth": GS_DEPTH_Z, "disparity": GS_DEPTH_DISPARITY, "relative_disparity": GS_DEPTH_RELATIVE_DISPARITY,
+               "log": GS_DEPTH_LOG}
 GS_ADAPTER_DETERMINISTIC = 1
 GS_TUNE_FORCE_RADIX_BINNING = 1
 GS_TUNE_NO_SPECULATION = 2
@@ -46,7 +53,7 @@ class GsConfig(Structure):
         ("near_cull_z", c_float), ("dilation", c_float), ("guard_band", c_float),
         ("sh_eval_max_degree", c_int32), ("tuning", c_uint32),
         ("viewmatrix", c_void_p), ("projmatrix", c_void_p), ("campos", c_void_p), ("bg", c_void_p),
-        ("tanfov", c_void_p), ("view_scale", c_void_p),
+        ("tanfov", c_void_p), ("view_scale", c_void_p), ("depth_mode", c_int32), ("depth_near_far", c_void_p),
     ]
 
 

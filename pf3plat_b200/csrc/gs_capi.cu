@@ -131,6 +131,17 @@ int validate(const GsConfig *cfg, const GsInputs *in) {
     return GS_OK;
 }
 
+// The forward's depth mode (GsConfig::depth_mode): known, on a depth channel, with the near / far its f(z) reads.
+int validate_depth_mode(const GsConfig *cfg) {
+    const int m = cfg->depth_mode;
+    if (m < GS_DEPTH_Z || m > GS_DEPTH_LOG) return gs_set_error(GS_ERR_INVALID, "unknown depth_mode");
+    if (m != GS_DEPTH_Z && !(cfg->flags & GS_FLAG_DEPTH))
+        return gs_set_error(GS_ERR_INVALID, "a depth_mode other than GS_DEPTH_Z needs GS_FLAG_DEPTH");
+    if ((m == GS_DEPTH_RELATIVE_DISPARITY || m == GS_DEPTH_LOG) && !cfg->depth_near_far)
+        return gs_set_error(GS_ERR_INVALID, "depth_mode GS_DEPTH_RELATIVE_DISPARITY / GS_DEPTH_LOG needs depth_near_far");
+    return GS_OK;
+}
+
 DevCfg make_dev_cfg(const GsConfig *cfg) {
     DevCfg c{};
     c.P = cfg->P; c.S = cfg->S; c.V = cfg->V; c.VPS = cfg->V / cfg->S; c.M = cfg->M;
@@ -326,6 +337,7 @@ struct FwdCall {
     const HostFeed *feed;
     void *radii_dst; size_t radii_bytes;  // gs_render_host: host destination of the radii
     uint32_t tuning;
+    DepthMode dm;                         // what the depth channel composites (launch_preprocess: rec2.w = f(z))
     int pre_variant, composite_variant;   // launch_preprocess / launch_composite_fwd variants
     bool split_colour, merge_sort;        // k_sh_colour on the aux stream; GS_TUNE_STRATA_MERGE_SORT
     // scratch: rects[n] | counters | cursors | verdict words | sub-bucket offsets | tile_start | tile_n
@@ -422,7 +434,7 @@ int FwdCall::speculate(SpecState &spec, const BinShape &shape, const BinPlan &pl
         for (int k = 0; k < (pieces ? pieces : 1); k++) {
             if (pieces) FWD_CUDA(cudaStreamWaitEvent(st, ctx->feed_ev[k], 0), "cudaStreamWaitEvent(feed)");
             FWD_OK(launch_preprocess(c, di, s->rec0, s->rec1, s->rec2, s->meta, out->radii, rects, emit, st,
-                                     pieces ? feed->begin[k] : 0, pieces ? feed->begin[k + 1] : -1, pre_variant));
+                                     pieces ? feed->begin[k] : 0, pieces ? feed->begin[k + 1] : -1, pre_variant, dm));
         }
     }
     if (!plan.fused_emit)
@@ -493,7 +505,7 @@ int FwdCall::exact(SpecState &spec, const BinShape &shape, GrowBuf &tabs) {
         const PreEmit emit{tile_counts, nullptr, 0, nullptr, 0};  // sub-bucket = index % BIN_SUB
         for (int k = 0; feed && k < feed->chunks; k++)  // gs_render_host: every piece of the SH block must have landed
             FWD_CUDA(cudaStreamWaitEvent(st, ctx->feed_ev[k], 0), "cudaStreamWaitEvent(feed)");
-        FWD_OK(launch_preprocess(c, di, s->rec0, s->rec1, s->rec2, s->meta, out->radii, rects, emit, st, 0, -1, pre_variant));
+        FWD_OK(launch_preprocess(c, di, s->rec0, s->rec1, s->rec2, s->meta, out->radii, rects, emit, st, 0, -1, pre_variant, dm));
         ctx->stats.kernel_launches += (c.P > 0);
     }
     uint32_t max_count;   // longest tile list
@@ -549,6 +561,7 @@ int forward(GsContext *ctx, const GsConfig *cfg, const GsInputs *in, const GsOut
     if (rc != GS_OK) return rc;
     if (!out->color || (cfg->P > 0 && !out->radii)) return gs_set_error(GS_ERR_INVALID, "color/radii outputs missing");
     if ((cfg->flags & GS_FLAG_DEPTH) && !out->depth) return gs_set_error(GS_ERR_INVALID, "GS_FLAG_DEPTH needs out->depth");
+    if ((rc = validate_depth_mode(cfg)) != GS_OK) return rc;
     FwdCall f{};
     f.ctx = ctx; f.c = make_dev_cfg(cfg); f.di = make_dev_inputs(in); f.out = out; f.st = st; f.feed = feed;
     const DevCfg &c = f.c;
@@ -561,6 +574,7 @@ int forward(GsContext *ctx, const GsConfig *cfg, const GsInputs *in, const GsOut
 
     // kernel variants (gs_render_host with a pinned SH block: geometry-only preprocess, colours in k_sh_colour)
     f.tuning = cfg->tuning;
+    f.dm = DepthMode{cfg->depth_mode, cfg->depth_near_far};
     const bool zero_copy = feed && feed->sh_zero_copy;
     f.split_colour = zero_copy && !(f.tuning & GS_TUNE_NO_SPLIT_COLOUR) && n > 0 && sh_colour_supported(c, f.di);
     f.pre_variant = ((f.tuning & GS_TUNE_PRE_OCC6) ? 1 : 0) | (((f.tuning & GS_TUNE_PRE_SH_RAW16) || zero_copy) ? 2 : 0) |
@@ -585,6 +599,7 @@ int forward(GsContext *ctx, const GsConfig *cfg, const GsInputs *in, const GsOut
         return gs_set_cuda_error(e, "cudaMallocAsync(saved)", __FILE__, __LINE__);
     }
     saved_layout(s, c, static_cast<unsigned char *>(s->base));
+    s->depth_mode = cfg->depth_mode;   // (the compositor reads it)
     if (f.split_colour && (rc = f.start_colour()) != GS_OK) return f.fail(rc);
 
     bool committed = false;
@@ -624,6 +639,10 @@ extern "C" int gs_backward(GsContext *ctx, const GsConfig *cfg, const GsInputs *
     c.flags = saved->flags;
     if (gin->dL_dviewmatrix_z && !(c.flags & GS_FLAG_DEPTH))
         return gs_set_error(GS_ERR_INVALID, "dL_dviewmatrix_z needs a forward with GS_FLAG_DEPTH");
+    // the forward's depth mode, with this call's near / far
+    const DepthMode dm{saved->depth_mode, cfg->depth_near_far};
+    if ((dm.mode == GS_DEPTH_RELATIVE_DISPARITY || dm.mode == GS_DEPTH_LOG) && !dm.near_far)
+        return gs_set_error(GS_ERR_INVALID, "the forward's depth_mode needs depth_near_far in the backward too");
     const bool det = (cfg->flags & GS_FLAG_DETERMINISTIC) != 0;
     if (det) {
         if (cfg->tuning & GS_TUNE_BWD_V1)
@@ -667,7 +686,7 @@ extern "C" int gs_backward(GsContext *ctx, const GsConfig *cfg, const GsInputs *
     }
     {
         StageTimer t(ctx, GS_STAGE_PREPROCESS_BWD, st);
-        rc = launch_preprocess_bwd(c, di, *saved, acc, g, st, (cfg->tuning & GS_TUNE_PBWD_2PHASE) ? 1 : 0, da);
+        rc = launch_preprocess_bwd(c, di, *saved, acc, g, st, (cfg->tuning & GS_TUNE_PBWD_2PHASE) ? 1 : 0, da, dm);
         if (rc != GS_OK) return rc;
     }
     ctx->stats.kernel_launches += 2;  // k_composite_bwd, k_preprocess_bwd
@@ -692,6 +711,7 @@ extern "C" int gs_render_host(GsContext *ctx, const GsConfig *cfg, const GsInput
     if (!ctx || !out) return gs_set_error(GS_ERR_INVALID, "null context/outputs");
     int rc = validate(cfg, in);
     if (rc != GS_OK) return rc;
+    if ((rc = validate_depth_mode(cfg)) != GS_OK) return rc;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     const size_t SP = (size_t)cfg->S * cfg->P, VP = (size_t)cfg->V * cfg->P, V = (size_t)cfg->V;
     const size_t px = V * cfg->image_height * cfg->image_width;
@@ -725,6 +745,7 @@ extern "C" int gs_render_host(GsContext *ctx, const GsConfig *cfg, const GsInput
         {cfg->bg, cfg->bg ? V * 12 : 0, (const void **)&dc.bg},
         {cfg->tanfov, cfg->tanfov ? V * 8 : 0, (const void **)&dc.tanfov},
         {cfg->view_scale, cfg->view_scale ? V * 4 : 0, (const void **)&dc.view_scale},
+        {cfg->depth_near_far, cfg->depth_near_far ? V * 8 : 0, (const void **)&dc.depth_near_far},
         {in->means3D, SP * 12, (const void **)&din.means3D},
         {in->opacities, SP * 4, (const void **)&din.opacities},
         {in->shs, (in->shs && !sh_alias) ? SP * cfg->M * 12 : 0, (const void **)&din.shs},

@@ -4,8 +4,9 @@
 // V*P entries each, written by preprocess and gathered by the compositors with 16-byte loads:
 //   rec0 = (x_pix, y_pix, -0.5*log2e*conic_a, -log2e*conic_b)
 //   rec1 = (-0.5*log2e*conic_c, opacity, r, g)
-//   rec2 = (b, z_cam, reach2, 0)      reach2 = -(log2(255*opacity) + margin): a pixel can receive the Gaussian
-//                                     only where log2 G >= reach2 (see gs_box_reaches)
+//   rec2 = (b, z_cam, reach2, fz)     reach2 = -(log2(255*opacity) + margin): a pixel can receive the Gaussian
+//                                     only where log2 G >= reach2 (see gs_box_reaches); fz = f(z) of a depth mode
+//                                     other than GS_DEPTH_Z (the value its depth channel composites), else 0
 // The conic is stored pre-scaled so that the compositors get log2(G) = power*log2(e) with five FP ops and feed
 // it straight to ex2.approx (gs_power2 / gs_ex2 below; forward and backward share them bit for bit).
 // plus meta[V*P] (uint8: bits 0-2 = SH clamp flags, bit 3 = visible).
@@ -33,6 +34,13 @@ struct DevInputs {
     const float *means3D, *opacities, *shs, *colors_precomp, *scales, *rotations, *cov3D;
 };
 
+// Depth mode of the depth channel (GsConfig::depth_mode).  Passed to the kernels as a trailing parameter of its own
+// (DevCfg's layout, and with it every other kernel's parameter offsets, stays as it was).
+struct DepthMode {
+    int mode;                    // GS_DEPTH_*
+    const float *near_far;       // device [V,2] unscaled (near, far), or NULL when the mode reads neither
+};
+
 // State a forward keeps for its backward; one stream-ordered allocation carved into planes.
 struct GsSaved {
     void *base;
@@ -48,6 +56,7 @@ struct GsSaved {
     int P, S, V, H, W;
     uint32_t flags;
     int has_sh, has_scales;
+    int depth_mode;               // GS_DEPTH_* of the forward (its backward chains the same f'(z))
 };
 
 #define GS_CUDA_OK(call)                                                             \
@@ -75,7 +84,8 @@ struct PreEmit {
 int launch_preprocess(const DevCfg &c, const DevInputs &in, float4 *rec0, float4 *rec1, float4 *rec2, uint8_t *meta,
                       int32_t *radii, ushort4 *rects, const PreEmit &emit, cudaStream_t st, int g_begin = 0,
                       int g_end = -1 /* = P */,
-                      int variant = 0 /* bit 0: 80 registers, 6 CTAs/SM (GS_TUNE_PRE_OCC6); bit 1: M > 16 rows staged as 16-byte pieces at their own stride (zero-copy feed, GS_TUNE_PRE_SH_RAW16); bit 2: geometry only, colour words left to k_sh_colour */);
+                      int variant = 0 /* bit 0: 80 registers, 6 CTAs/SM (GS_TUNE_PRE_OCC6); bit 1: M > 16 rows staged as 16-byte pieces at their own stride (zero-copy feed, GS_TUNE_PRE_SH_RAW16); bit 2: geometry only, colour words left to k_sh_colour */,
+                      const DepthMode &dm = DepthMode{} /* mode != GS_DEPTH_Z: rec2.w = f(z) (the FZ kernels) */);
 // the colour words (rec1.zw, rec2.x) of every (view, Gaussian) from the SH block -- gs_render_host's split pipeline
 bool sh_colour_supported(const DevCfg &c, const DevInputs &in);
 int launch_sh_colour(const DevCfg &c, const DevInputs &in, float4 *rec1, float4 *rec2, uint8_t *clamp_out /* [V*P] or NULL */, cudaStream_t st);
@@ -121,15 +131,18 @@ struct DetAcc {
     float *view_z;            // [V][warps of one scene's preprocess-backward grid][4] (needs no zeroing)
 };
 
+// GS_FLAG_DEPTH: the depth channel composites rec2.y (s.depth_mode == GS_DEPTH_Z) or rec2.w (any other mode); the backward
+// compositors take the same word for the depth term of dL/dalpha
 int launch_composite_fwd(const DevCfg &c, const GsSaved &s, float *color, float *depth, cudaStream_t st,
                          int variant = 0 /* 2: the persistent warp-specialised kernel (GS_TUNE_FWD_WS) */);
 int launch_composite_bwd(const DevCfg &c, const GsSaved &s, const float *dL_dcolor, const float *dL_ddepth,
                          float *grad_acc /* [V*P*GS_ACC_STRIDE], zeroed */, cudaStream_t st,
                          int variant = 0 /* 1: the round-1 kernel (GS_TUNE_BWD_V1) */,
                          const DetAcc &det = DetAcc{} /* det.acc != NULL: fixed-point accumulators instead of grad_acc */);
+// s.depth_mode != GS_DEPTH_Z: the depth gradient is chained through f'(z) (dm.near_far: the backward call's array)
 int launch_preprocess_bwd(const DevCfg &c, const DevInputs &in, const GsSaved &s, const float *grad_acc,
                           const GsInGrads &g, cudaStream_t st, int variant = 0 /* 1: the two-phase kernel (GS_TUNE_PBWD_2PHASE) */,
-                          const DetAcc &det = DetAcc{});
+                          const DetAcc &det = DetAcc{}, const DepthMode &dm = DepthMode{});
 // bytes of DetAcc::view_z for a configuration
 size_t det_view_z_bytes(const DevCfg &c);
 
@@ -296,6 +309,30 @@ __device__ __forceinline__ float gs_rcp(float x) {
     float y;
     asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
     return y;
+}
+
+// Depth modes other than GS_DEPTH_Z (render_depth_cuda, cuda_splatting.py:245-251, with depth_to_relative_disparity of
+// conversions.py:17-27 in its own expression order): the fake colour f at the UNSCALED depth z, and the factor
+// f'(z) * dz/dz_s that carries dL/df onto the view-scaled depth z_s = s z the kernels work with.  IEEE division (the
+// default '/'); the mode is a uniform runtime branch.
+#define GS_DEPTH_EPS 1e-10f
+__device__ __forceinline__ float gs_depth_f(int mode, float z, float near_, float far_) {
+    if (mode == GS_DEPTH_DISPARITY) return 1.0f / z;
+    if (mode == GS_DEPTH_RELATIVE_DISPARITY) {
+        const float d = 1.0f / (z + GS_DEPTH_EPS), dn = 1.0f / (near_ + GS_DEPTH_EPS), df = 1.0f / (far_ + GS_DEPTH_EPS);
+        return 1.0f - (d - df) / (dn - df + GS_DEPTH_EPS);
+    }
+    return logf(fmaxf(fminf(z, near_), far_));   // GS_DEPTH_LOG, the clamp as written
+}
+__device__ __forceinline__ float gs_depth_chain(int mode, float zs, float s, float near_, float far_) {
+    const float z = zs / s;
+    if (mode == GS_DEPTH_DISPARITY) return -1.0f / (z * z) / s;
+    if (mode == GS_DEPTH_RELATIVE_DISPARITY) {
+        const float dn = 1.0f / (near_ + GS_DEPTH_EPS), df = 1.0f / (far_ + GS_DEPTH_EPS), ze = z + GS_DEPTH_EPS;
+        return 1.0f / (ze * ze * (dn - df + GS_DEPTH_EPS)) / s;
+    }
+    // GS_DEPTH_LOG: d/dz log(max(min(z, near), far)) = 1/z where z passes both clamps (never, for near < far)
+    return (z < near_ && z > far_) ? 1.0f / z / s : 0.0f;
 }
 
 #define GS_SH_C0 0.28209479177387814f

@@ -40,7 +40,8 @@ struct PixState {
 };
 
 // Returns whether this pixel received the Gaussian (and hence wrote non-trivial partial gradients to g).
-template <bool DEPTH>
+// DEPTH: as k_composite_fwd (2: the depth value is rec2.w)
+template <int DEPTH>
 __device__ __forceinline__ bool pixel_grad(PixState &ps, bool live, uint32_t rec_addr, float pxf, float pyf,
                                            float half_w, float half_h, float *g /* [GS_ACC_STRIDE] */) {
 #pragma unroll
@@ -69,9 +70,10 @@ __device__ __forceinline__ bool pixel_grad(PixState &ps, bool live, uint32_t rec
         g[ch] = w * ps.dLp[ch];
     }
     if (DEPTH) {
+        const float dz = DEPTH == 2 ? lds32(rec_addr + 44u) : q2.y;
         ps.accum_d = fmaf(ps.last_alpha, ps.last_d, keep * ps.accum_d);
-        ps.last_d = q2.y;
-        dL_dalpha = fmaf(q2.y - ps.accum_d, ps.dLd, dL_dalpha);
+        ps.last_d = dz;
+        dL_dalpha = fmaf(dz - ps.accum_d, ps.dLd, dL_dalpha);
         g[9] = w * ps.dLd;
     }
     ps.last_alpha = alpha;
@@ -92,7 +94,7 @@ __device__ __forceinline__ bool pixel_grad(PixState &ps, bool live, uint32_t rec
     return true;
 }
 
-template <bool DEPTH, int CB_BATCH, int MINB>
+template <int DEPTH, int CB_BATCH, int MINB>
 __global__ void __launch_bounds__(CB_THREADS, MINB)
 k_composite_bwd_v1(const DevCfg c, const float4 *__restrict__ rec0, const float4 *__restrict__ rec1,
                 const float4 *__restrict__ rec2, const uint32_t *__restrict__ point_list,
@@ -285,8 +287,9 @@ struct Cb2Smem {
 // on the order of the tile list -- are added into exact fixed-point accumulators (gs_det.cuh) with 64-bit integer REDs
 // instead of float REDs, so the totals do not depend on the order in which warps arrive.  A term with no encoding
 // (non-finite, out of range) sets its component's bit in the poison mask.  DET = false is the default kernel,
-// instruction for instruction (the two trailing parameters are unused).
-template <bool DEPTH, int CB_BATCH, int MINB, bool DET = false>
+// instruction for instruction (the two trailing parameters are unused).  DEPTH: as k_composite_fwd (2: the depth term of
+// dL/dalpha takes rec2.w).
+template <int DEPTH, int CB_BATCH, int MINB, bool DET = false>
 __global__ void __launch_bounds__(CB_THREADS, MINB)
 k_composite_bwd(const DevCfg c, const float4 *__restrict__ rec0, const float4 *__restrict__ rec1,
                 const float4 *__restrict__ rec2, const uint32_t *__restrict__ point_list,
@@ -491,7 +494,7 @@ k_composite_bwd(const DevCfg c, const float4 *__restrict__ rec0, const float4 *_
                     T *= inv;
                     ws.x = alpha * T;
                     float cdot = fmaf(q2.x, dl.z, fmaf(q1.w, dl.y, q1.z * dl.x));
-                    if (DEPTH) cdot = fmaf(q2.y, dl.w, cdot);
+                    if (DEPTH) cdot = fmaf(DEPTH == 2 ? lds32(a + 44u) : q2.y, dl.w, cdot);
                     ws.y = fmaf(T, cdot, -(Y * inv)) * G;   // dL/dalpha * G (the gradient passes through the 0.99 clamp)
                     Y = fmaf(ws.x, cdot, Y);
                 }
@@ -529,15 +532,20 @@ int launch_composite_bwd(const DevCfg &c, const GsSaved &s, const float *dL_dcol
         };
         const bool dep = (c.flags & GS_FLAG_DEPTH) != 0;
         int rc;
-        if (det.acc) {
-            if (variant == 2)
-                rc = dep ? launch(k_composite_bwd<true, 128, 4, true>, sizeof(Cb2Smem<128>)) : launch(k_composite_bwd<false, 128, 4, true>, sizeof(Cb2Smem<128>));
+        if (dep && s.depth_mode != GS_DEPTH_Z) {   // the depth channel carried f(z) in rec2.w
+            if (det.acc)
+                rc = variant == 2 ? launch(k_composite_bwd<2, 128, 4, true>, sizeof(Cb2Smem<128>)) : launch(k_composite_bwd<2, 256, 3, true>, sizeof(Cb2Smem<256>));
             else
-                rc = dep ? launch(k_composite_bwd<true, 256, 3, true>, sizeof(Cb2Smem<256>)) : launch(k_composite_bwd<false, 256, 3, true>, sizeof(Cb2Smem<256>));
+                rc = variant == 2 ? launch(k_composite_bwd<2, 128, 4>, sizeof(Cb2Smem<128>)) : launch(k_composite_bwd<2, 256, 3>, sizeof(Cb2Smem<256>));
+        } else if (det.acc) {
+            if (variant == 2)
+                rc = dep ? launch(k_composite_bwd<1, 128, 4, true>, sizeof(Cb2Smem<128>)) : launch(k_composite_bwd<0, 128, 4, true>, sizeof(Cb2Smem<128>));
+            else
+                rc = dep ? launch(k_composite_bwd<1, 256, 3, true>, sizeof(Cb2Smem<256>)) : launch(k_composite_bwd<0, 256, 3, true>, sizeof(Cb2Smem<256>));
         } else if (variant == 2)
-            rc = dep ? launch(k_composite_bwd<true, 128, 4>, sizeof(Cb2Smem<128>)) : launch(k_composite_bwd<false, 128, 4>, sizeof(Cb2Smem<128>));
+            rc = dep ? launch(k_composite_bwd<1, 128, 4>, sizeof(Cb2Smem<128>)) : launch(k_composite_bwd<0, 128, 4>, sizeof(Cb2Smem<128>));
         else
-            rc = dep ? launch(k_composite_bwd<true, 256, 3>, sizeof(Cb2Smem<256>)) : launch(k_composite_bwd<false, 256, 3>, sizeof(Cb2Smem<256>));
+            rc = dep ? launch(k_composite_bwd<1, 256, 3>, sizeof(Cb2Smem<256>)) : launch(k_composite_bwd<0, 256, 3>, sizeof(Cb2Smem<256>));
         if (rc != GS_OK) return rc;
         GS_CUDA_OK(cudaGetLastError());
         return GS_OK;
@@ -553,7 +561,9 @@ int launch_composite_bwd(const DevCfg &c, const GsSaved &s, const float *dL_dcol
                                              dL_dcolor, dL_ddepth, grad_acc);
         return GS_OK;
     };
-    const int rc = (c.flags & GS_FLAG_DEPTH) ? launch(k_composite_bwd_v1<true, BATCH, MINB>) : launch(k_composite_bwd_v1<false, BATCH, MINB>);
+    const int rc = !(c.flags & GS_FLAG_DEPTH) ? launch(k_composite_bwd_v1<0, BATCH, MINB>)
+                   : s.depth_mode == GS_DEPTH_Z ? launch(k_composite_bwd_v1<1, BATCH, MINB>)
+                                                 : launch(k_composite_bwd_v1<2, BATCH, MINB>);
     if (rc != GS_OK) return rc;
     GS_CUDA_OK(cudaGetLastError());
     return GS_OK;

@@ -33,7 +33,9 @@ struct CfStage {
     float4 rec[CF_BATCH][3];
 };
 
-template <bool DEPTH, int MINB>
+// DEPTH: 0 no depth channel; 1 the channel composites rec2.y (GS_DEPTH_Z); 2 it composites rec2.w, the f(z) preprocess
+// stored for the other depth modes.  Values 0 and 1 are the kernels of before, instruction for instruction.
+template <int DEPTH, int MINB>
 __global__ void __launch_bounds__(CF_THREADS, MINB)
 k_composite_fwd(const DevCfg c, const float4 *__restrict__ rec0, const float4 *__restrict__ rec1,
                 const float4 *__restrict__ rec2, const uint32_t *__restrict__ point_list,
@@ -121,7 +123,7 @@ k_composite_fwd(const DevCfg c, const float4 *__restrict__ rec0, const float4 *_
                         C0 = fmaf(q1.z, w, C0);
                         C1 = fmaf(q1.w, w, C1);
                         C2 = fmaf(q2.x, w, C2);
-                        if (DEPTH) Dz = fmaf(q2.y, w, Dz);
+                        if (DEPTH) Dz = fmaf(DEPTH == 2 ? lds32(a + 44u) : q2.y, w, Dz);
                         T = test_T;
                         last = pos0 + chunk + bit;
                     }
@@ -188,7 +190,7 @@ __device__ __forceinline__ uint32_t ld_volatile_shared(const uint32_t *p) {
     return v;
 }
 
-template <bool DEPTH, int MINB>
+template <int DEPTH, int MINB>   // DEPTH as k_composite_fwd
 __global__ void __launch_bounds__(CP_THREADS, MINB)
 k_composite_fwd_ws(const DevCfg c, const float4 *__restrict__ rec0, const float4 *__restrict__ rec1,
                    const float4 *__restrict__ rec2, const uint32_t *__restrict__ point_list,
@@ -314,7 +316,7 @@ k_composite_fwd_ws(const DevCfg c, const float4 *__restrict__ rec0, const float4
                                 C0 = fmaf(q1.z, w, C0);
                                 C1 = fmaf(q1.w, w, C1);
                                 C2 = fmaf(q2.x, w, C2);
-                                if (DEPTH) Dz = fmaf(q2.y, w, Dz);
+                                if (DEPTH) Dz = fmaf(DEPTH == 2 ? lds32(a + 44u) : q2.y, w, Dz);
                                 T = test_T;
                                 last = pos0 + chunk + bit;
                             }
@@ -356,23 +358,24 @@ int launch_composite_fwd(const DevCfg &c, const GsSaved &s, float *color, float 
         static int ctas_per_device[64] = {};   // per device: SM count x occupancy of the kernel
         int dev = 0;
         GS_CUDA_OK(cudaGetDevice(&dev));
-        const bool with_depth = (c.flags & GS_FLAG_DEPTH) != 0;
+        const int depth_kind = !(c.flags & GS_FLAG_DEPTH) ? 0 : (s.depth_mode == GS_DEPTH_Z ? 1 : 2);
         if (dev >= 0 && dev < 64 && ctas_per_device[dev] == 0) {
             int sms = 0, per_sm = 0;
             GS_CUDA_OK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-            GS_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_composite_fwd_ws<false, MINB_WS>, CP_THREADS, 0));
+            GS_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_composite_fwd_ws<0, MINB_WS>, CP_THREADS, 0));
             ctas_per_device[dev] = sms * (per_sm > 0 ? per_sm : 1);
         }
         const uint32_t total = (uint32_t)c.ntiles * (uint32_t)c.V;
         const uint32_t resident = (dev >= 0 && dev < 64) ? (uint32_t)ctas_per_device[dev] : 132u * MINB_WS;
         const uint32_t nctas = total < resident ? total : resident;
         GS_CUDA_OK(cudaMemsetAsync(s.sched, 0, 8, st));
-        if (with_depth)
-            k_composite_fwd_ws<true, MINB_WS><<<nctas, CP_THREADS, 0, st>>>(c, s.rec0, s.rec1, s.rec2, s.point_list, s.ranges, color, depth,
-                                                                        s.final_T, s.n_contrib, s.sched, total);
-        else
-            k_composite_fwd_ws<false, MINB_WS><<<nctas, CP_THREADS, 0, st>>>(c, s.rec0, s.rec1, s.rec2, s.point_list, s.ranges, color, depth,
-                                                                         s.final_T, s.n_contrib, s.sched, total);
+        auto launch_ws = [&](auto kern) {
+            kern<<<nctas, CP_THREADS, 0, st>>>(c, s.rec0, s.rec1, s.rec2, s.point_list, s.ranges, color, depth, s.final_T,
+                                               s.n_contrib, s.sched, total);
+        };
+        if (depth_kind == 2) launch_ws(k_composite_fwd_ws<2, MINB_WS>);
+        else if (depth_kind == 1) launch_ws(k_composite_fwd_ws<1, MINB_WS>);
+        else launch_ws(k_composite_fwd_ws<0, MINB_WS>);
         GS_CUDA_OK(cudaGetLastError());
         return GS_OK;
     }
@@ -383,8 +386,9 @@ int launch_composite_fwd(const DevCfg &c, const GsSaved &s, float *color, float 
     auto launch = [&](auto kern) {
         kern<<<grid, CF_THREADS, 0, st>>>(c, s.rec0, s.rec1, s.rec2, s.point_list, s.ranges, color, depth, s.final_T, s.n_contrib);
     };
-    if (c.flags & GS_FLAG_DEPTH) launch(k_composite_fwd<true, MINB>);
-    else launch(k_composite_fwd<false, MINB>);
+    if (!(c.flags & GS_FLAG_DEPTH)) launch(k_composite_fwd<0, MINB>);
+    else if (s.depth_mode == GS_DEPTH_Z) launch(k_composite_fwd<1, MINB>);
+    else launch(k_composite_fwd<2, MINB>);
     GS_CUDA_OK(cudaGetLastError());
     return GS_OK;
 }

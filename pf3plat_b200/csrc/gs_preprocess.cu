@@ -43,6 +43,7 @@ struct PreSmem {
     ViewCam cams[GS_CAM_CHUNK];
     float strata[GS_CAM_CHUNK][BIN_SUB];  // depth-stratum boundaries of the staged views (PreEmit::strata)
     uint64_t bar;
+    float2 near_far[GS_CAM_CHUNK];        // unscaled (near, far) of the staged views (FZ kernels only; inside the padding)
 };
 constexpr int PRE_SMEM_HDR = (sizeof(PreSmem) + 127) / 128 * 128;
 
@@ -136,6 +137,13 @@ __device__ __forceinline__ float3 sh_view_dir(float3 m, const float *campos) {
     return make_float3(__fmul_rn(dx, inv), __fmul_rn(dy, inv), __fmul_rn(dz, inv));
 }
 
+// FZ kernels: the unscaled (near, far) of views [v0, v0 + count) next to their cameras (all threads; the caller's barrier
+// follows).  Modes that read neither may come without the array.
+__device__ __forceinline__ void stage_near_far(const DepthMode &dm, int v0, int count, float2 *dst) {
+    for (int t = threadIdx.x; t < count; t += blockDim.x)
+        dst[t] = dm.near_far ? make_float2(dm.near_far[(v0 + t) * 2], dm.near_far[(v0 + t) * 2 + 1]) : make_float2(0.f, 0.f);
+}
+
 // Everything preprocess derives for one (view, Gaussian).
 struct Splat {
     float4 r0, r1, r2;
@@ -208,11 +216,14 @@ __device__ __forceinline__ void project_splat(const DevCfg &c, const ViewCam &ca
 // MINB: resident CTAs per SM the register allocation is bounded for.  Unbounded the kernel takes 96 registers (5 CTAs/SM;
 // latency-bound).  Bounded to 64 (8 CTAs/SM, 116 bytes of spills and more instructions) it was slower on C2.
 // B4: degree-4 evaluation (25 coefficients staged per Gaussian); the B4 = false kernels are the degree-<=3 ones unchanged.
-template <int COLOUR, int MINB, bool B4 = false>
+// FZ: a depth mode other than GS_DEPTH_Z -- rec2.w = f(z) of dm.mode (a uniform runtime branch), with the views' near and
+// far staged next to their cameras.  The FZ = false kernels are the ones without it, instruction for instruction (dm unused).
+template <int COLOUR, int MINB, bool B4 = false, bool FZ = false>
 __global__ void __launch_bounds__(PRE_THREADS, MINB)
 k_preprocess(const DevCfg c, const DevInputs in, float4 *__restrict__ rec0, float4 *__restrict__ rec1,
              float4 *__restrict__ rec2, uint8_t *__restrict__ meta, int32_t *__restrict__ radii,
-             ushort4 *__restrict__ rects, const PreEmit emit, const int g_begin, const int g_end, const int sh_raw16) {
+             ushort4 *__restrict__ rects, const PreEmit emit, const int g_begin, const int g_end, const int sh_raw16,
+             const DepthMode dm) {
     extern __shared__ __align__(128) unsigned char smem_raw[];
     PreSmem *sm = reinterpret_cast<PreSmem *>(smem_raw);
     float *sh_s = reinterpret_cast<float *>(smem_raw + PRE_SMEM_HDR);
@@ -312,6 +323,7 @@ k_preprocess(const DevCfg c, const DevInputs in, float4 *__restrict__ rec0, floa
         if (emit.strata && !emit.strata_per_tile)
             for (int t = tid; t < nv * BIN_SUB; t += PRE_THREADS)
                 sm->strata[t / BIN_SUB][t % BIN_SUB] = emit.strata[(size_t)(scene * c.VPS) * BIN_SUB + t];
+        if (FZ) stage_near_far(dm, scene * c.VPS, nv, sm->near_far);
     }
     if (HAS_SH) {
         cp_async_wait<0>();  // this thread's share of the strided copy (no-op on the other paths)
@@ -345,6 +357,7 @@ k_preprocess(const DevCfg c, const DevInputs in, float4 *__restrict__ rec0, floa
             if (emit.strata && !emit.strata_per_tile)
                 for (int t = tid; t < nv * BIN_SUB; t += PRE_THREADS)
                     sm->strata[t / BIN_SUB][t % BIN_SUB] = emit.strata[(size_t)(scene * c.VPS + v0) * BIN_SUB + t];
+            if (FZ) stage_near_far(dm, scene * c.VPS + v0, nv, sm->near_far);
             __syncthreads();
         }
         if (!active) continue;
@@ -354,6 +367,9 @@ k_preprocess(const DevCfg c, const DevInputs in, float4 *__restrict__ rec0, floa
             Splat sp;
             project_splat<COLOUR, B4>(c, sm->cams[vi], mean, c6, opac, sh_s + (size_t)tid * RS,
                                   COLOUR == 1 ? in.colors_precomp + o * 3 : nullptr, sp);
+            // the depth channel's value: f at the unscaled depth z = z_s / s
+            if (FZ && sp.radius > 0)
+                sp.r2.w = gs_depth_f(dm.mode, sp.r2.y / sm->cams[vi].scale, sm->near_far[vi].x, sm->near_far[vi].y);
             // fused speculative emission: nothing reads the rects afterwards (k_emit_buckets and the strata learning, their
             // readers, run on the other paths only)
             const bool fused = emit.counters && emit.bucket;
@@ -543,7 +559,7 @@ __global__ void k_mark_visible(const DevCfg c, const float *__restrict__ means3D
 
 int launch_preprocess(const DevCfg &c, const DevInputs &in, float4 *rec0, float4 *rec1, float4 *rec2, uint8_t *meta,
                       int32_t *radii, ushort4 *rects, const PreEmit &emit, cudaStream_t st, int g_begin, int g_end,
-                      int variant) {
+                      int variant, const DepthMode &dm) {
     if (g_end < 0) g_end = c.P;
     if (g_end <= g_begin) return GS_OK;
     const bool more_ctas = (variant & 1) != 0;
@@ -564,11 +580,16 @@ int launch_preprocess(const DevCfg &c, const DevInputs &in, float4 *rec0, float4
     if (smem > (size_t)227 * 1024) return gs_set_error(GS_ERR_INVALID, "too many SH coefficients per Gaussian for the staging buffer");
     auto launch = [&](auto kern) -> int {
         GS_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        kern<<<grid, PRE_THREADS, smem, st>>>(c, in, rec0, rec1, rec2, meta, radii, rects, emit, g_begin, g_end, sh_raw16);
+        kern<<<grid, PRE_THREADS, smem, st>>>(c, in, rec0, rec1, rec2, meta, radii, rects, emit, g_begin, g_end, sh_raw16, dm);
         return GS_OK;
     };
     int rc;
-    if (variant & 4) rc = more_ctas ? launch(k_preprocess<0, 6>) : launch(k_preprocess<0, 5>);   // geometry only
+    if (dm.mode != GS_DEPTH_Z) {   // rec2.w = f(z): the FZ kernels
+        if (variant & 4) rc = more_ctas ? launch(k_preprocess<0, 6, false, true>) : launch(k_preprocess<0, 5, false, true>);
+        else if (b4) rc = launch(k_preprocess<2, 5, true, true>);
+        else if (in.shs) rc = more_ctas ? launch(k_preprocess<2, 6, false, true>) : launch(k_preprocess<2, 5, false, true>);
+        else rc = more_ctas ? launch(k_preprocess<1, 6, false, true>) : launch(k_preprocess<1, 5, false, true>);
+    } else if (variant & 4) rc = more_ctas ? launch(k_preprocess<0, 6>) : launch(k_preprocess<0, 5>);   // geometry only
     else if (b4) rc = launch(k_preprocess<2, 5, true>);
     else if (in.shs) rc = more_ctas ? launch(k_preprocess<2, 6>) : launch(k_preprocess<2, 5>);
     else rc = more_ctas ? launch(k_preprocess<1, 6>) : launch(k_preprocess<1, 5>);

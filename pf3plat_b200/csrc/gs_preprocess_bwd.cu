@@ -161,6 +161,15 @@ __device__ __forceinline__ void view_z_grad(const GsInGrads &g, const DetAcc &de
     }
 }
 
+// VIEW_Z = 2 kernels: the depth channel carried f(z) of dm.mode, so the accumulated gz = sum alpha T dL/ddepth is dL/df,
+// and f'(z) dz/dz_s (this factor) carries it onto the view-scaled depth z_s, recomputed exactly as preprocess computed it.
+__device__ __forceinline__ float depth_chain(const ViewCam &cam, float3 mean, const DepthMode &dm, int v) {
+    const float s = cam.scale;
+    const float zs = xform4x3(cam.view, make_float3(mean.x * s, mean.y * s, mean.z * s)).z;
+    const float nr = dm.near_far ? dm.near_far[v * 2] : 0.f, fr = dm.near_far ? dm.near_far[v * 2 + 1] : 0.f;
+    return gs_depth_chain(dm.mode, zs, s, nr, fr);
+}
+
 // The decoded fixed-point accumulators of (view, Gaussian) o (deterministic mode), written to out; returns out.
 __device__ __forceinline__ const float *load_det_acc(const DetAcc &det, size_t o, float out[GS_ACC_STRIDE]) {
     const uint32_t bad = det.poison[o];
@@ -170,17 +179,19 @@ __device__ __forceinline__ const float *load_det_acc(const DetAcc &det, size_t o
     return out;
 }
 
-// VIEW_Z: also write g.dL_dviewmatrix_z, the depth channel's gradient w.r.t. the z column of each view matrix
+// VIEW_Z: 1 also write g.dL_dviewmatrix_z, the depth channel's gradient w.r.t. the z column of each view matrix
 // (z = view[2] m.x + view[6] m.y + view[10] m.z + view[14], m the view-scaled mean).  The default instantiations
-// (VIEW_Z = false) are the kernels without it, instruction for instruction.  DET: the accumulators are the fixed-point
-// ones of the deterministic backward (det.acc, det.poison) and the view-matrix gradient goes through det.view_z.
+// (VIEW_Z = 0) are the kernels without it, instruction for instruction.  2: the forward's depth mode was not GS_DEPTH_Z --
+// the depth gradient is chained through f'(z) of dm.mode, and the view-matrix gradient is written if g asks for it.
+// DET: the accumulators are the fixed-point ones of the deterministic backward (det.acc, det.poison) and the view-matrix
+// gradient goes through det.view_z.
 // B4: degree 4 (c.deg == 4, M >= 25).  The 48 accumulators of bands 0..3 stay in registers as in the default kernel; the
 // 27 of band 4 live in a shared-memory row per thread next to the staged inputs (stride 27, odd: conflict-free), which
 // keeps the register bound -- and so the 4 resident CTAs per SM -- of the default kernel.
-template <bool HAS_SH, int MINB, bool VIEW_Z = false, bool DET = false, bool B4 = false>
+template <bool HAS_SH, int MINB, int VIEW_Z = 0, bool DET = false, bool B4 = false>
 __global__ void __launch_bounds__(PB_THREADS, MINB)
 k_preprocess_bwd(const DevCfg c, const DevInputs in, const uint8_t *__restrict__ meta, const float *__restrict__ acc,
-                    const GsInGrads g, const DetAcc det) {
+                    const GsInGrads g, const DetAcc det, const DepthMode dm) {
     extern __shared__ __align__(128) unsigned char smem_raw[];
     PbSmem *sm = reinterpret_cast<PbSmem *>(smem_raw);
     float *sh_s = reinterpret_cast<float *>(smem_raw + PB_SMEM_HDR);
@@ -252,14 +263,14 @@ k_preprocess_bwd(const DevCfg c, const DevInputs in, const uint8_t *__restrict__
             __syncthreads();
         }
         if (!active) {
-            if (VIEW_Z) view_z_grad<DET>(g, det, v, 0.f, 0.f, 0.f, 0.f);
+            if (VIEW_Z == 1 || (VIEW_Z == 2 && g.dL_dviewmatrix_z)) view_z_grad<DET>(g, det, v, 0.f, 0.f, 0.f, 0.f);
             continue;
         }
         const ViewCam &cam = sm->cams[vi % GS_CAM_CHUNK];
         const size_t o = (size_t)v * c.P + i;
         const uint32_t mb = meta[o];
         float m2d[2] = {0.f, 0.f}, gcol[3] = {0.f, 0.f, 0.f};
-        if (VIEW_Z && !(mb & GS_META_VISIBLE)) view_z_grad<DET>(g, det, v, 0.f, 0.f, 0.f, 0.f);
+        if ((VIEW_Z == 1 || (VIEW_Z == 2 && g.dL_dviewmatrix_z)) && !(mb & GS_META_VISIBLE)) view_z_grad<DET>(g, det, v, 0.f, 0.f, 0.f, 0.f);
         if (mb & GS_META_VISIBLE) {
             const float *a = acc + o * GS_ACC_STRIDE;
             float a_det[GS_ACC_STRIDE];
@@ -268,7 +279,7 @@ k_preprocess_bwd(const DevCfg c, const DevInputs in, const uint8_t *__restrict__
             m2d[0] = a[3]; m2d[1] = a[4];
             const float gcx = a[5], gcy = a[6], gcz = a[7];
             gopac += a[8];
-            const float gz = a[9];
+            const float gz = VIEW_Z == 2 ? a[9] * depth_chain(cam, mean, dm, v) : a[9];
             const float s = cam.scale, s2 = s * s;
             const float3 m = make_float3(mean.x * s, mean.y * s, mean.z * s);
             const float cv[6] = {c6[0] * s2, c6[1] * s2, c6[2] * s2, c6[3] * s2, c6[4] * s2, c6[5] * s2};
@@ -334,7 +345,7 @@ k_preprocess_bwd(const DevCfg c, const DevInputs in, const uint8_t *__restrict__
             gm[0] += cam.view[2] * gz;
             gm[1] += cam.view[6] * gz;
             gm[2] += cam.view[10] * gz;
-            if (VIEW_Z) view_z_grad<DET>(g, det, v, gz * m.x, gz * m.y, gz * m.z, gz);
+            if (VIEW_Z == 1 || (VIEW_Z == 2 && g.dL_dviewmatrix_z)) view_z_grad<DET>(g, det, v, gz * m.x, gz * m.y, gz * m.z, gz);
             // ---- colour -> SH coefficients and mean (view direction) ----
             if (HAS_SH) {
                 const float d[3] = {m.x - cam.campos[0], m.y - cam.campos[1], m.z - cam.campos[2]};
@@ -468,10 +479,10 @@ k_preprocess_bwd(const DevCfg c, const DevInputs in, const uint8_t *__restrict__
 // camera / direction / basis work is redone per phase), and slower.  The single-pass kernel stays the default.
 constexpr int PB2_MIN_CTAS = 6;
 
-template <bool HAS_SH, bool VIEW_Z = false, bool DET = false>
+template <bool HAS_SH, int VIEW_Z = 0, bool DET = false>   // VIEW_Z as k_preprocess_bwd
 __global__ void __launch_bounds__(PB_THREADS, PB2_MIN_CTAS)
 k_preprocess_bwd_2phase(const DevCfg c, const DevInputs in, const uint8_t *__restrict__ meta, const float *__restrict__ acc,
-                 const GsInGrads g, const DetAcc det) {
+                 const GsInGrads g, const DetAcc det, const DepthMode dm) {
     extern __shared__ __align__(128) unsigned char smem_raw[];
     PbSmem *sm = reinterpret_cast<PbSmem *>(smem_raw);
     float *sh_s = reinterpret_cast<float *>(smem_raw + PB_SMEM_HDR);
@@ -546,14 +557,14 @@ k_preprocess_bwd_2phase(const DevCfg c, const DevInputs in, const uint8_t *__res
                 __syncthreads();
             }
             if (!active) {
-                if (VIEW_Z) view_z_grad<DET>(g, det, v, 0.f, 0.f, 0.f, 0.f);
+                if (VIEW_Z == 1 || (VIEW_Z == 2 && g.dL_dviewmatrix_z)) view_z_grad<DET>(g, det, v, 0.f, 0.f, 0.f, 0.f);
                 continue;
             }
             const ViewCam &cam = sm->cams[vi % GS_CAM_CHUNK];
             const size_t o = (size_t)v * c.P + i;
             const uint32_t mb = meta[o];
             float m2d[2] = {0.f, 0.f}, gcol[3] = {0.f, 0.f, 0.f};
-            if (VIEW_Z && !(mb & GS_META_VISIBLE)) view_z_grad<DET>(g, det, v, 0.f, 0.f, 0.f, 0.f);
+            if ((VIEW_Z == 1 || (VIEW_Z == 2 && g.dL_dviewmatrix_z)) && !(mb & GS_META_VISIBLE)) view_z_grad<DET>(g, det, v, 0.f, 0.f, 0.f, 0.f);
             if (mb & GS_META_VISIBLE) {
                 const float *a = acc + o * GS_ACC_STRIDE;
                 float a_det[GS_ACC_STRIDE];
@@ -562,7 +573,7 @@ k_preprocess_bwd_2phase(const DevCfg c, const DevInputs in, const uint8_t *__res
                 m2d[0] = a[3]; m2d[1] = a[4];
                 const float gcx = a[5], gcy = a[6], gcz = a[7];
                 gopac += a[8];
-                const float gz = a[9];
+                const float gz = VIEW_Z == 2 ? a[9] * depth_chain(cam, mean, dm, v) : a[9];
                 const float s = cam.scale, s2 = s * s;
                 const float3 m = make_float3(mean.x * s, mean.y * s, mean.z * s);
                 const float cv[6] = {c6[0] * s2, c6[1] * s2, c6[2] * s2, c6[3] * s2, c6[4] * s2, c6[5] * s2};
@@ -628,7 +639,7 @@ k_preprocess_bwd_2phase(const DevCfg c, const DevInputs in, const uint8_t *__res
                 gm[0] += cam.view[2] * gz;
                 gm[1] += cam.view[6] * gz;
                 gm[2] += cam.view[10] * gz;
-                if (VIEW_Z) view_z_grad<DET>(g, det, v, gz * m.x, gz * m.y, gz * m.z, gz);
+                if (VIEW_Z == 1 || (VIEW_Z == 2 && g.dL_dviewmatrix_z)) view_z_grad<DET>(g, det, v, gz * m.x, gz * m.y, gz * m.z, gz);
 #pragma unroll
                 for (int k = 0; k < 3; k++) gmean[k] += s * gm[k];
             }
@@ -757,9 +768,9 @@ k_preprocess_bwd_2phase(const DevCfg c, const DevInputs in, const uint8_t *__res
     }
 }
 
-template <bool VIEW_Z, bool DET>
+template <int VIEW_Z, bool DET>
 int launch_preprocess_bwd_t(const DevCfg &c, const DevInputs &in, const GsSaved &s, const float *grad_acc,
-                            const GsInGrads &g, cudaStream_t st, int variant, const DetAcc &det) {
+                            const GsInGrads &g, cudaStream_t st, int variant, const DetAcc &det, const DepthMode &dm) {
     dim3 grid((c.P + PB_THREADS - 1) / PB_THREADS, c.S);
     if (in.shs && c.deg > 3) {   // degree 4: the single-pass kernel with band 4 compiled in
         if (variant == 1)
@@ -767,21 +778,21 @@ int launch_preprocess_bwd_t(const DevCfg &c, const DevInputs &in, const GsSaved 
         const size_t smem = PB_SMEM_HDR + (size_t)PB_THREADS * (c.M * 3 + PB_SH_B4) * 4;
         auto kern = k_preprocess_bwd<true, PB_MIN_CTAS, VIEW_Z, DET, true>;
         GS_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        kern<<<grid, PB_THREADS, smem, st>>>(c, in, s.meta, grad_acc, g, det);
+        kern<<<grid, PB_THREADS, smem, st>>>(c, in, s.meta, grad_acc, g, det, dm);
     } else if (variant != 1) {  // single pass over the views (default)
         if (in.shs) {
             size_t smem = PB_SMEM_HDR + (size_t)PB_THREADS * c.M * 12;
             GS_CUDA_OK(cudaFuncSetAttribute(k_preprocess_bwd<true, PB_MIN_CTAS, VIEW_Z, DET>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-            k_preprocess_bwd<true, PB_MIN_CTAS, VIEW_Z, DET><<<grid, PB_THREADS, smem, st>>>(c, in, s.meta, grad_acc, g, det);
+            k_preprocess_bwd<true, PB_MIN_CTAS, VIEW_Z, DET><<<grid, PB_THREADS, smem, st>>>(c, in, s.meta, grad_acc, g, det, dm);
         } else {
-            k_preprocess_bwd<false, PB_MIN_CTAS, VIEW_Z, DET><<<grid, PB_THREADS, PB_SMEM_HDR, st>>>(c, in, s.meta, grad_acc, g, det);
+            k_preprocess_bwd<false, PB_MIN_CTAS, VIEW_Z, DET><<<grid, PB_THREADS, PB_SMEM_HDR, st>>>(c, in, s.meta, grad_acc, g, det, dm);
         }
     } else if (in.shs) {
         size_t smem = PB_SMEM_HDR + (size_t)PB_THREADS * (c.M <= PB_SH_EVAL ? c.M * 3 : PB_SH_EVAL * 3 + 1) * 4;
         GS_CUDA_OK(cudaFuncSetAttribute(k_preprocess_bwd_2phase<true, VIEW_Z, DET>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        k_preprocess_bwd_2phase<true, VIEW_Z, DET><<<grid, PB_THREADS, smem, st>>>(c, in, s.meta, grad_acc, g, det);
+        k_preprocess_bwd_2phase<true, VIEW_Z, DET><<<grid, PB_THREADS, smem, st>>>(c, in, s.meta, grad_acc, g, det, dm);
     } else {
-        k_preprocess_bwd_2phase<false, VIEW_Z, DET><<<grid, PB_THREADS, PB_SMEM_HDR, st>>>(c, in, s.meta, grad_acc, g, det);
+        k_preprocess_bwd_2phase<false, VIEW_Z, DET><<<grid, PB_THREADS, PB_SMEM_HDR, st>>>(c, in, s.meta, grad_acc, g, det, dm);
     }
     GS_CUDA_OK(cudaGetLastError());
     return GS_OK;
@@ -807,14 +818,20 @@ size_t det_view_z_bytes(const DevCfg &c) { return (size_t)c.V * view_z_warps(c) 
 // g.dL_dviewmatrix_z non-NULL selects the VIEW_Z kernels; the caller has zeroed it (the kernels accumulate into it, or in
 // deterministic mode k_view_z_finalize writes it).  det.acc non-NULL selects the deterministic kernels.
 int launch_preprocess_bwd(const DevCfg &c, const DevInputs &in, const GsSaved &s, const float *grad_acc,
-                          const GsInGrads &g, cudaStream_t st, int variant, const DetAcc &det) {
+                          const GsInGrads &g, cudaStream_t st, int variant, const DetAcc &det, const DepthMode &dm) {
     if (c.P == 0) return GS_OK;
-    if (!det.acc)
-        return g.dL_dviewmatrix_z ? launch_preprocess_bwd_t<true, false>(c, in, s, grad_acc, g, st, variant, det)
-                                  : launch_preprocess_bwd_t<false, false>(c, in, s, grad_acc, g, st, variant, det);
-    if (!g.dL_dviewmatrix_z) return launch_preprocess_bwd_t<false, true>(c, in, s, grad_acc, g, st, variant, det);
-    const int rc = launch_preprocess_bwd_t<true, true>(c, in, s, grad_acc, g, st, variant, det);
-    if (rc != GS_OK) return rc;
+    // a forward whose depth channel carried f(z): the VIEW_Z = 2 kernels, with or without the view-matrix gradient
+    const bool fz = (s.flags & GS_FLAG_DEPTH) && s.depth_mode != GS_DEPTH_Z;
+    if (!det.acc) {
+        if (fz) return launch_preprocess_bwd_t<2, false>(c, in, s, grad_acc, g, st, variant, det, dm);
+        return g.dL_dviewmatrix_z ? launch_preprocess_bwd_t<1, false>(c, in, s, grad_acc, g, st, variant, det, dm)
+                                  : launch_preprocess_bwd_t<0, false>(c, in, s, grad_acc, g, st, variant, det, dm);
+    }
+    int rc;
+    if (fz) rc = launch_preprocess_bwd_t<2, true>(c, in, s, grad_acc, g, st, variant, det, dm);
+    else if (!g.dL_dviewmatrix_z) return launch_preprocess_bwd_t<0, true>(c, in, s, grad_acc, g, st, variant, det, dm);
+    else rc = launch_preprocess_bwd_t<1, true>(c, in, s, grad_acc, g, st, variant, det, dm);
+    if (rc != GS_OK || !g.dL_dviewmatrix_z) return rc;
     k_view_z_finalize<<<(c.V * 4 + 127) / 128, 128, 0, st>>>(c.V, view_z_warps(c), det.view_z, g.dL_dviewmatrix_z);
     GS_CUDA_OK(cudaGetLastError());
     return GS_OK;

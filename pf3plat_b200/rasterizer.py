@@ -168,6 +168,10 @@ class BatchSettings(NamedTuple):
     # highest SH degree evaluated (GsConfig.sh_eval_max_degree): 3, or 4 to evaluate and train band 4 of a 25-coefficient
     # block; None = the process-wide setting (set_sh_eval_max_degree)
     sh_eval_max_degree: Optional[int] = None
+    # what the depth channel (with_depth) composites: PF3plat's DepthRenderingMode -- "depth" (camera-space z of the
+    # view-scaled scene), "disparity", "relative_disparity" or "log" (f(z) of render_depth_cuda at the unscaled z)
+    depth_mode: str = "depth"
+    depth_near_far: Optional[torch.Tensor] = None  # (V,2) unscaled near, far: needed by "relative_disparity" and "log"
 
 
 # ---------------------------------------------------------------------------------------------------------
@@ -216,11 +220,15 @@ def _make_config(bs: BatchSettings, S: int, P: int, M: int, keep: list) -> GsCon
     cfg.scale_modifier = float(bs.scale_modifier)
     cfg.tuning = int(bs.tuning)
     cfg.sh_eval_max_degree = _check_degree(_sh_eval_max_degree if bs.sh_eval_max_degree is None else bs.sh_eval_max_degree)
+    if bs.depth_mode not in _capi.DEPTH_MODES:
+        raise ValueError(f"depth_mode must be one of {sorted(_capi.DEPTH_MODES)}, got {bs.depth_mode!r}")
+    cfg.depth_mode = _capi.DEPTH_MODES[bs.depth_mode]
     tensors = {
         "viewmatrix": _f32c(bs.viewmatrix).reshape(V, 16), "projmatrix": _f32c(bs.projmatrix, dev).reshape(V, 16),
         "campos": _f32c(bs.campos, dev).reshape(V, 3), "bg": _f32c(bs.bg, dev).reshape(V, 3),
         "tanfov": None if bs.tanfov is None else _f32c(bs.tanfov, dev).reshape(V, 2),
         "view_scale": None if bs.view_scale is None else _f32c(bs.view_scale, dev).reshape(V),
+        "depth_near_far": None if bs.depth_near_far is None else _f32c(bs.depth_near_far, dev).reshape(V, 2),
     }
     for k, t in tensors.items():
         setattr(cfg, k, _ptr(t))

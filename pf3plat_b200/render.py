@@ -3,8 +3,8 @@
 
 Replaces, behind the same argument meaning:
   * `render_cuda`        PF3plat's src/model/decoder/cuda_splatting.py:47-127
-  * `render_depth_cuda`  PF3plat's src/model/decoder/cuda_splatting.py:226-269 (mode "depth" fused as a
-                         4th composited channel; other modes render the fake colour like the reference)
+  * `render_depth_cuda`  PF3plat's src/model/decoder/cuda_splatting.py:226-269 (every DepthRenderingMode fused as a
+                         4th composited channel; `render_depth` keeps the reference's second render to compare against)
   * the body of `DecoderSplattingCUDA.forward`  PF3plat's src/model/decoder/decoder_splatting_cuda.py:35-67
 All views of all scenes go through ONE gs_forward call (one host sync per batch instead of three per view).
 """
@@ -33,13 +33,15 @@ def _cov6(cov: torch.Tensor) -> torch.Tensor:
 def render_views(extrinsics, intrinsics, near, far, image_shape, background_color, gaussian_means,
                  gaussian_covariances, gaussian_sh_coefficients, gaussian_opacities, scale_invariant: bool = True,
                  use_sh: bool = True, with_depth: bool = False, sh_layout: str = "g_xyz_n",
-                 sh_eval_max_degree: Optional[int] = None):
+                 sh_eval_max_degree: Optional[int] = None, depth_mode: str = "depth"):
     """extrinsics (B,4,4) c2w, intrinsics (B,3,3), near/far (B,), background (B,3); Gaussians are per SCENE and NOT
     repeated per view: means (S,G,3), covariances (S,G,3,3) or (S,G,6), sh (S,G,3,d_sh) [or (S,G,d_sh,3) with
     sh_layout="g_n_xyz"], opacities (S,G); B % S == 0 and view b shows scene b // (B//S).
     sh_eval_max_degree: highest SH degree evaluated (3, or 4 for band 4 of d_sh = 25); None = the process-wide setting
     (rasterizer.set_sh_eval_max_degree, default 3).
-    Returns color (B,3,h,w) and, if with_depth, depth (B,h,w) = sum_i alpha_i T_i z_i."""
+    Returns color (B,3,h,w) and, if with_depth, depth (B,h,w) = sum_i alpha_i T_i f(z_i): f(z) = z of the (rescaled)
+    scene for depth_mode "depth"; for "disparity", "relative_disparity" and "log" the fake colour of render_depth_cuda
+    (cuda_splatting.py:245-251) at the UNSCALED camera-space depth z, with the unscaled near and far."""
     assert use_sh or gaussian_sh_coefficients.shape[-1 if sh_layout == "g_xyz_n" else -2] == 1
     h, w = image_shape
     vb = make_view_batch(extrinsics, intrinsics, near, far, scale_invariant)
@@ -55,7 +57,8 @@ def render_views(extrinsics, intrinsics, near, far, image_shape, background_colo
     bs = BatchSettings(image_height=h, image_width=w, viewmatrix=vb.viewmatrix, projmatrix=vb.projmatrix,
                        campos=vb.campos, bg=background_color, sh_degree=degree, tanfov=vb.tanfov,
                        view_scale=vb.scale if scale_invariant else None, with_depth=with_depth,
-                       sh_eval_max_degree=sh_eval_max_degree)
+                       sh_eval_max_degree=sh_eval_max_degree, depth_mode=depth_mode,
+                       depth_near_far=torch.stack([near, far], -1) if with_depth and depth_mode != "depth" else None)
     B = extrinsics.shape[0]
     S = gaussian_means.shape[0]
     if use_sh:
@@ -80,41 +83,38 @@ def render_cuda(extrinsics, intrinsics, near, far, image_shape, background_color
 def decoder_forward(means, covariances, harmonics, opacities, extrinsics, intrinsics, near, far, image_shape,
                     background_color, depth_mode: Optional[str] = None, sh_eval_max_degree: Optional[int] = None):
     """`DecoderSplattingCUDA.forward` (decoder_splatting_cuda.py:35-67) without the v-fold repeat: Gaussians
-    (b,g,...), cameras (b,v,...).  Returns (color (b,v,3,h,w), depth (b,v,h,w) or None).  depth_mode "depth" is
-    fused into the colour pass; the reference's other modes are served by `render_depth`.
+    (b,g,...), cameras (b,v,...).  Returns (color (b,v,3,h,w), depth (b,v,h,w) or None).  Every depth_mode of the
+    reference ("depth", "disparity", "relative_disparity", "log") is composited in the same pass as the colour.
 
     Gradients: like the reference's colour pass, the colour gives the CAMERAS no gradient.  The reference's depth
     pass builds its fake colour z = (extrinsics^-1 @ mean).z in torch (cuda_splatting.py:239-242), so its depth is
     differentiable w.r.t. the extrinsics -- PF3plat trains with depth_mode "depth" on predicted poses.  The fused
-    channel gives exactly that gradient and no other: dL/ddepth reaches the z column of each view matrix
-    (make_view_batch carries it on to the extrinsics), besides the Gaussians.  A loss that does not read the depth
-    leaves the extrinsics without a gradient, as the reference does.  So "depth" is one render whether or not the
-    extrinsics require grad.  sh_eval_max_degree: as render_views."""
+    channel gives exactly that gradient and no other: dL/ddepth reaches the z column of each view matrix through the
+    mode's f'(z) (make_view_batch carries it on to the extrinsics), besides the Gaussians.  "log" clamps z as the
+    reference does, to the constant log(far) when near < far: its extrinsics get a zero gradient.  A loss that does not
+    read the depth leaves the extrinsics without a gradient, as the reference does.  So every mode is one render whether
+    or not the extrinsics require grad.  sh_eval_max_degree: as render_views."""
     b, v = extrinsics.shape[:2]
     flat = lambda t: t.reshape(b * v, *t.shape[2:])
     bg = background_color.reshape(1, 3).expand(b * v, 3)
-    if depth_mode is None or depth_mode == "depth":
-        out = render_views(flat(extrinsics), flat(intrinsics), flat(near), flat(far), image_shape, bg, means,
-                           covariances, harmonics, opacities, with_depth=depth_mode is not None,
-                           sh_eval_max_degree=sh_eval_max_degree)
-        if depth_mode is None:
-            return out.reshape(b, v, *out.shape[1:]), None
-        color, depth = out
+    out = render_views(flat(extrinsics), flat(intrinsics), flat(near), flat(far), image_shape, bg, means,
+                       covariances, harmonics, opacities, with_depth=depth_mode is not None,
+                       sh_eval_max_degree=sh_eval_max_degree, depth_mode=depth_mode or "depth")
+    if depth_mode is None:
+        return out.reshape(b, v, *out.shape[1:]), None
+    color, depth = out
+    if depth_mode == "depth":
         # the reference renders depth in the 1/near-rescaled scene (render_depth_cuda -> render_cuda with
         # scale_invariant=True) but takes the fake colour from the UNSCALED camera-space z
-        # (cuda_splatting.py:239-242): undo the rescale of z
+        # (cuda_splatting.py:239-242): undo the rescale of z (the other modes evaluate f at the unscaled z already)
         depth = depth * flat(near)[:, None, None]
-        return color.reshape(b, v, *color.shape[1:]), depth.reshape(b, v, *depth.shape[1:])
-    color = render_views(flat(extrinsics), flat(intrinsics), flat(near), flat(far), image_shape, bg, means,
-                         covariances, harmonics, opacities, sh_eval_max_degree=sh_eval_max_degree)
-    depth = render_depth(means, covariances, opacities, extrinsics, intrinsics, near, far, image_shape, depth_mode)
-    return color.reshape(b, v, *color.shape[1:]), depth
+    return color.reshape(b, v, *color.shape[1:]), depth.reshape(b, v, *depth.shape[1:])
 
 
 def render_depth(means, covariances, opacities, extrinsics, intrinsics, near, far, image_shape, mode: str = "depth"):
     """`render_depth_cuda` (cuda_splatting.py:226-269) for (b,g,...) Gaussians and (b,v,...) cameras: a second render
-    whose colour is the fake colour.  `decoder_forward` uses it for the modes other than "depth"; for "depth" it is the
-    reference's two-pass route, kept to compare the fused channel against."""
+    whose colour is the fake colour.  The reference's two-pass route for every mode, kept to compare the fused channel
+    of `decoder_forward` against."""
     b, v = extrinsics.shape[:2]
     flat = lambda t: t.reshape(b * v, *t.shape[2:])
     ext, nr, fr = flat(extrinsics), flat(near), flat(far)

@@ -172,6 +172,17 @@ typedef struct GsInGrads {
     float *dL_dviewmatrix_z;
 } GsInGrads;
 
+/* Accumulated opacity, the opt-in third image of the colour pass: alpha = 1 - T_final per pixel, with the T_final the
+ * colour composites the background with (same 1/255 threshold, 0.99 clamp and early stop), exactly 0 where nothing
+ * contributes.  Its gradient reaches means, 2-D means, covariances or scales / rotations and opacities; SH, colours and
+ * cameras get nothing from it.  Taken by the _ex entry points below (GsOutputs and GsOutGrads keep their layout). */
+typedef struct GsAlpha {
+    float *alpha;            /* gs_forward_ex: device [V,H,W]; gs_render_host_ex: host [V,H,W].  Required there; ignored
+                                by gs_backward_ex */
+    const float *dL_dalpha;  /* gs_backward_ex: device [V,H,W], or NULL (the gradients of gs_backward, bit for bit);
+                                ignored by the forward entries */
+} GsAlpha;
+
 /* Counters of the last forward on a context (host-visible after the call returns). */
 typedef struct GsStats {
     int64_t num_rendered;  /* tile instances after culling (the "D" of SURVEY.md section 8(d)) */
@@ -215,6 +226,16 @@ GS_API int gs_forward(GsContext *ctx, const GsConfig *cfg, const GsInputs *in, c
 GS_API int gs_backward(GsContext *ctx, const GsConfig *cfg, const GsInputs *in, const GsSaved *saved,
                 const GsOutGrads *gout, const GsInGrads *gin, void *stream);
 
+/* gs_forward that also writes the accumulated opacity to alpha->alpha (GsAlpha).  Colour, depth and radii are the
+ * bytes gs_forward writes, and the saved state is the same: either backward entry takes it. */
+GS_API int gs_forward_ex(GsContext *ctx, const GsConfig *cfg, const GsInputs *in, const GsOutputs *out,
+                         const GsAlpha *alpha, GsSaved **saved, void *stream);
+
+/* gs_backward with an incoming gradient of the accumulated opacity (alpha->dL_dalpha, may be NULL).  Works on the
+ * saved state of either forward entry: the opacity is 1 - the T_final every forward saves. */
+GS_API int gs_backward_ex(GsContext *ctx, const GsConfig *cfg, const GsInputs *in, const GsSaved *saved,
+                          const GsOutGrads *gout, const GsAlpha *alpha, const GsInGrads *gin, void *stream);
+
 GS_API void gs_saved_free(GsContext *ctx, GsSaved *saved, void *stream);
 
 /* GaussianRasterizer.markVisible (unused by PF3plat; kept for surface completeness): present[V,P] = in frustum. */
@@ -232,6 +253,10 @@ GS_API int gs_get_stats(const GsContext *ctx, GsStats *out);
  * does: the call synchronises).  Pageable or unaligned blocks are uploaded by the copy engine; results are identical.
  */
 GS_API int gs_render_host(GsContext *ctx, const GsConfig *cfg, const GsInputs *in, const GsOutputs *out, void *stream);
+/* gs_render_host that also returns the accumulated opacity in the HOST buffer alpha->alpha, from every feed (written
+ * directly by the compositor under GS_TUNE_DIRECT_OUTPUT when that buffer is pinned). */
+GS_API int gs_render_host_ex(GsContext *ctx, const GsConfig *cfg, const GsInputs *in, const GsOutputs *out,
+                             const GsAlpha *alpha, void *stream);
 
 /*
  * PSNR per image = compute_psnr of PF3plat's src/evaluation/metrics.py:11-19 (clip to [0,1], mean squared error

@@ -76,6 +76,11 @@ class GsInGrads(Structure):
                 ("dL_dcov3D", c_void_p), ("dL_dviewmatrix_z", c_void_p)]
 
 
+class GsAlpha(Structure):
+    """The accumulated-opacity output of gs_forward_ex / gs_render_host_ex and its incoming gradient of gs_backward_ex."""
+    _fields_ = [("alpha", c_void_p), ("dL_dalpha", c_void_p)]
+
+
 class GsStats(Structure):
     _fields_ = [("num_rendered", c_int64), ("num_visible", c_int64), ("saved_bytes", c_int64),
                 ("scratch_bytes", c_int64), ("kernel_launches", c_int32), ("max_tile_list", c_int32),
@@ -133,6 +138,12 @@ SYMBOLS = {
     "gs_mark_visible": (c_int, [c_void_p, POINTER(GsConfig), c_void_p, c_void_p, c_void_p]),
     "gs_get_stats": (c_int, [c_void_p, POINTER(GsStats)]),
     "gs_render_host": (c_int, [c_void_p, POINTER(GsConfig), POINTER(GsInputs), POINTER(GsOutputs), c_void_p]),
+    "gs_forward_ex": (c_int, [c_void_p, POINTER(GsConfig), POINTER(GsInputs), POINTER(GsOutputs), POINTER(GsAlpha),
+                              POINTER(c_void_p), c_void_p]),
+    "gs_backward_ex": (c_int, [c_void_p, POINTER(GsConfig), POINTER(GsInputs), c_void_p, POINTER(GsOutGrads),
+                               POINTER(GsAlpha), POINTER(GsInGrads), c_void_p]),
+    "gs_render_host_ex": (c_int, [c_void_p, POINTER(GsConfig), POINTER(GsInputs), POINTER(GsOutputs), POINTER(GsAlpha),
+                                  c_void_p]),
     "gs_set_profiling": (c_int, [c_void_p, c_int]),
     "gs_get_stage_ms": (c_int, [c_void_p, POINTER(c_float)]),
     "gs_psnr_scratch_floats": (c_int64, [c_int32, c_int64]),

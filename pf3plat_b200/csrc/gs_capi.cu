@@ -333,6 +333,7 @@ struct FwdCall {
     DevCfg c;
     DevInputs di;
     const GsOutputs *out;
+    float *alpha;                         // gs_forward_ex / gs_render_host_ex: accumulated opacity [V*H*W], else null
     cudaStream_t st;
     const HostFeed *feed;
     void *radii_dst; size_t radii_bytes;  // gs_render_host: host destination of the radii
@@ -393,7 +394,7 @@ struct FwdCall {
             colour_pending = false;
             FWD_CUDA(cudaStreamWaitEvent(st, ctx->ev_colour, 0), "cudaStreamWaitEvent(colour)");
         }
-        return timed(GS_STAGE_COMPOSITE, [&] { return launch_composite_fwd(c, *s, out->color, out->depth, st, composite_variant); });
+        return timed(GS_STAGE_COMPOSITE, [&] { return launch_composite_fwd(c, *s, out->color, out->depth, st, composite_variant, alpha); });
     }
 };
 
@@ -554,7 +555,7 @@ int FwdCall::exact(SpecState &spec, const BinShape &shape, GrowBuf &tabs) {
 #undef FWD_CUDA
 
 int forward(GsContext *ctx, const GsConfig *cfg, const GsInputs *in, const GsOutputs *out, GsSaved **saved_out,
-            cudaStream_t st, const HostFeed *feed) {
+            cudaStream_t st, const HostFeed *feed, float *alpha) {
     if (saved_out) *saved_out = nullptr;
     if (!ctx || !out) return gs_set_error(GS_ERR_INVALID, "null context/outputs");
     int rc = validate(cfg, in);
@@ -563,7 +564,7 @@ int forward(GsContext *ctx, const GsConfig *cfg, const GsInputs *in, const GsOut
     if ((cfg->flags & GS_FLAG_DEPTH) && !out->depth) return gs_set_error(GS_ERR_INVALID, "GS_FLAG_DEPTH needs out->depth");
     if ((rc = validate_depth_mode(cfg)) != GS_OK) return rc;
     FwdCall f{};
-    f.ctx = ctx; f.c = make_dev_cfg(cfg); f.di = make_dev_inputs(in); f.out = out; f.st = st; f.feed = feed;
+    f.ctx = ctx; f.c = make_dev_cfg(cfg); f.di = make_dev_inputs(in); f.out = out; f.alpha = alpha; f.st = st; f.feed = feed;
     const DevCfg &c = f.c;
     const size_t n = (size_t)c.V * c.P;
     const BinShape shape{c.V, c.ntiles, c.P, c.S};
@@ -623,11 +624,20 @@ int forward(GsContext *ctx, const GsConfig *cfg, const GsInputs *in, const GsOut
 
 extern "C" int gs_forward(GsContext *ctx, const GsConfig *cfg, const GsInputs *in, const GsOutputs *out,
                           GsSaved **saved_out, void *stream) {
-    return forward(ctx, cfg, in, out, saved_out, static_cast<cudaStream_t>(stream), nullptr);
+    return forward(ctx, cfg, in, out, saved_out, static_cast<cudaStream_t>(stream), nullptr, nullptr);
 }
 
-extern "C" int gs_backward(GsContext *ctx, const GsConfig *cfg, const GsInputs *in, const GsSaved *saved,
-                           const GsOutGrads *gout, const GsInGrads *gin, void *stream) {
+extern "C" int gs_forward_ex(GsContext *ctx, const GsConfig *cfg, const GsInputs *in, const GsOutputs *out,
+                             const GsAlpha *alpha, GsSaved **saved_out, void *stream) {
+    if (saved_out) *saved_out = nullptr;
+    if (!alpha) return gs_set_error(GS_ERR_INVALID, "null alpha request");
+    if (!alpha->alpha) return gs_set_error(GS_ERR_INVALID, "gs_forward_ex needs alpha->alpha (gs_forward renders without it)");
+    return forward(ctx, cfg, in, out, saved_out, static_cast<cudaStream_t>(stream), nullptr, alpha->alpha);
+}
+
+namespace {
+int backward(GsContext *ctx, const GsConfig *cfg, const GsInputs *in, const GsSaved *saved, const GsOutGrads *gout,
+             const float *dL_dalpha, const GsInGrads *gin, void *stream) {
     if (!ctx || !saved || !gout || !gin) return gs_set_error(GS_ERR_INVALID, "null argument");
     int rc = validate(cfg, in);
     if (rc != GS_OK) return rc;
@@ -681,7 +691,8 @@ extern "C" int gs_backward(GsContext *ctx, const GsConfig *cfg, const GsInputs *
     {
         StageTimer t(ctx, GS_STAGE_COMPOSITE_BWD, st);
         GS_CUDA_OK(cudaMemsetAsync(ctx->per_gaussian.p, 0, acc_bytes, st));
-        rc = launch_composite_bwd(c, *saved, gout->dL_dcolor, gout->dL_ddepth, acc, st, (cfg->tuning & GS_TUNE_BWD_V1) ? 1 : ((cfg->tuning & GS_TUNE_BWD_OCC4) ? 2 : 0), da);
+        rc = launch_composite_bwd(c, *saved, gout->dL_dcolor, gout->dL_ddepth, acc, st, (cfg->tuning & GS_TUNE_BWD_V1) ? 1 : ((cfg->tuning & GS_TUNE_BWD_OCC4) ? 2 : 0), da,
+                                  dL_dalpha);
         if (rc != GS_OK) return rc;
     }
     {
@@ -692,6 +703,18 @@ extern "C" int gs_backward(GsContext *ctx, const GsConfig *cfg, const GsInputs *
     ctx->stats.kernel_launches += 2;  // k_composite_bwd, k_preprocess_bwd
     if (det && g.dL_dviewmatrix_z) ctx->stats.kernel_launches += 1;  // k_view_z_finalize
     return GS_OK;
+}
+}  // namespace
+
+extern "C" int gs_backward(GsContext *ctx, const GsConfig *cfg, const GsInputs *in, const GsSaved *saved,
+                           const GsOutGrads *gout, const GsInGrads *gin, void *stream) {
+    return backward(ctx, cfg, in, saved, gout, nullptr, gin, stream);
+}
+
+extern "C" int gs_backward_ex(GsContext *ctx, const GsConfig *cfg, const GsInputs *in, const GsSaved *saved,
+                              const GsOutGrads *gout, const GsAlpha *alpha, const GsInGrads *gin, void *stream) {
+    if (!alpha) return gs_set_error(GS_ERR_INVALID, "null alpha request");
+    return backward(ctx, cfg, in, saved, gout, alpha->dL_dalpha, gin, stream);
 }
 
 extern "C" int gs_mark_visible(GsContext *ctx, const GsConfig *cfg, const float *means3D, uint8_t *present,
@@ -706,8 +729,10 @@ extern "C" int gs_mark_visible(GsContext *ctx, const GsConfig *cfg, const float 
 // ---------------------------------------------------------------------------------------------------------
 // end-to-end entry with host buffers
 // ---------------------------------------------------------------------------------------------------------
-extern "C" int gs_render_host(GsContext *ctx, const GsConfig *cfg, const GsInputs *in, const GsOutputs *out,
-                              void *stream) {
+namespace {
+// alpha_host: gs_render_host_ex's host buffer for the accumulated opacity, else null
+int render_host(GsContext *ctx, const GsConfig *cfg, const GsInputs *in, const GsOutputs *out, float *alpha_host,
+                void *stream) {
     if (!ctx || !out) return gs_set_error(GS_ERR_INVALID, "null context/outputs");
     int rc = validate(cfg, in);
     if (rc != GS_OK) return rc;
@@ -757,7 +782,7 @@ extern "C" int gs_render_host(GsContext *ctx, const GsConfig *cfg, const GsInput
     size_t total = 0;
     for (const Item &it : items) total += align256(it.bytes);
     const size_t out_off = total;
-    total += align256(px * 12) + align256(VP * 4) + align256(px * 4);
+    total += align256(px * 12) + align256(VP * 4) + align256(px * 4) + (alpha_host ? align256(px * 4) : 0);
     rc = ctx->host_stage.reserve(total, 1.0);
     if (rc != GS_OK) return rc;
     unsigned char *base = static_cast<unsigned char *>(ctx->host_stage.p);
@@ -814,6 +839,8 @@ extern "C" int gs_render_host(GsContext *ctx, const GsConfig *cfg, const GsInput
     dout.radii = reinterpret_cast<int32_t *>(base + out_off + align256(px * 12));
     dout.depth = (cfg->flags & GS_FLAG_DEPTH) ? reinterpret_cast<float *>(base + out_off + align256(px * 12) + align256(VP * 4))
                                               : nullptr;
+    float *dalpha = alpha_host ? reinterpret_cast<float *>(base + out_off + align256(px * 12) + align256(VP * 4) + align256(px * 4))
+                               : nullptr;
     // Experiment (GS_TUNE_DIRECT_OUTPUT): let the compositor write the images STRAIGHT into the caller's buffers when those
     // are pinned (device-accessible under unified addressing), instead of a device-to-host copy of the whole image queued
     // behind it (C2: 6.3 MB at the very end of the call).  In-process on C2 (scripts/ab_e2e.py) direct output was
@@ -824,7 +851,9 @@ extern "C" int gs_render_host(GsContext *ctx, const GsConfig *cfg, const GsInput
     void *depth_alias = direct && dout.depth ? device_alias(out->depth) : nullptr;
     if (color_alias) dout.color = static_cast<float *>(color_alias);
     if (depth_alias) dout.depth = static_cast<float *>(depth_alias);
-    rc = forward(ctx, &dc, &din, &dout, nullptr, st, &feed);
+    void *alpha_alias = direct && alpha_host ? device_alias(alpha_host) : nullptr;
+    if (alpha_alias) dalpha = static_cast<float *>(alpha_alias);
+    rc = forward(ctx, &dc, &din, &dout, nullptr, st, &feed, dalpha);
     if (rc != GS_OK) {
         // nothing of ours may still be reading the caller's buffers (the colour kernel pulls out of them) once we return
         if (ctx->aux_stream) cudaStreamSynchronize(ctx->aux_stream);
@@ -835,7 +864,21 @@ extern "C" int gs_render_host(GsContext *ctx, const GsConfig *cfg, const GsInput
     if (out->color && !color_alias) GS_CUDA_OK(cudaMemcpyAsync(out->color, dout.color, px * 12, cudaMemcpyDeviceToHost, st));
     if (out->depth && dout.depth && !depth_alias)
         GS_CUDA_OK(cudaMemcpyAsync(out->depth, dout.depth, px * 4, cudaMemcpyDeviceToHost, st));
+    if (alpha_host && !alpha_alias) GS_CUDA_OK(cudaMemcpyAsync(alpha_host, dalpha, px * 4, cudaMemcpyDeviceToHost, st));
     GS_CUDA_OK(cudaStreamSynchronize(st));
     GS_CUDA_OK(cudaStreamSynchronize(ctx->copy_stream));  // radii (started after the forward's mid-way sync)
     return GS_OK;
+}
+}  // namespace
+
+extern "C" int gs_render_host(GsContext *ctx, const GsConfig *cfg, const GsInputs *in, const GsOutputs *out,
+                              void *stream) {
+    return render_host(ctx, cfg, in, out, nullptr, stream);
+}
+
+extern "C" int gs_render_host_ex(GsContext *ctx, const GsConfig *cfg, const GsInputs *in, const GsOutputs *out,
+                                 const GsAlpha *alpha, void *stream) {
+    if (!alpha) return gs_set_error(GS_ERR_INVALID, "null alpha request");
+    if (!alpha->alpha) return gs_set_error(GS_ERR_INVALID, "gs_render_host_ex needs alpha->alpha (gs_render_host renders without it)");
+    return render_host(ctx, cfg, in, out, alpha->alpha, stream);
 }

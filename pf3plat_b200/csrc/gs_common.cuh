@@ -133,12 +133,16 @@ struct DetAcc {
 
 // GS_FLAG_DEPTH: the depth channel composites rec2.y (s.depth_mode == GS_DEPTH_Z) or rec2.w (any other mode); the backward
 // compositors take the same word for the depth term of dL/dalpha
+// alpha (GsAlpha): the forward also writes 1 - T_final per pixel ([V*H*W]); the backward takes dL/dalpha into the
+// background term of every dL/dalpha_i.  NULL: the kernels of before.
 int launch_composite_fwd(const DevCfg &c, const GsSaved &s, float *color, float *depth, cudaStream_t st,
-                         int variant = 0 /* 2: the persistent warp-specialised kernel (GS_TUNE_FWD_WS) */);
+                         int variant = 0 /* 2: the persistent warp-specialised kernel (GS_TUNE_FWD_WS) */,
+                         float *alpha = nullptr);
 int launch_composite_bwd(const DevCfg &c, const GsSaved &s, const float *dL_dcolor, const float *dL_ddepth,
                          float *grad_acc /* [V*P*GS_ACC_STRIDE], zeroed */, cudaStream_t st,
                          int variant = 0 /* 1: the round-1 kernel (GS_TUNE_BWD_V1) */,
-                         const DetAcc &det = DetAcc{} /* det.acc != NULL: fixed-point accumulators instead of grad_acc */);
+                         const DetAcc &det = DetAcc{} /* det.acc != NULL: fixed-point accumulators instead of grad_acc */,
+                         const float *dL_dalpha = nullptr);
 // s.depth_mode != GS_DEPTH_Z: the depth gradient is chained through f'(z) (dm.near_far: the backward call's array)
 int launch_preprocess_bwd(const DevCfg &c, const DevInputs &in, const GsSaved &s, const float *grad_acc,
                           const GsInGrads &g, cudaStream_t st, int variant = 0 /* 1: the two-phase kernel (GS_TUNE_PBWD_2PHASE) */,

@@ -12,6 +12,8 @@
 // warp total of value L, and ONE red.global.add.f32 instruction with 30 distinct addresses retires them:
 // one atomic instruction per three Gaussians per warp instead of 288 atomics.  (The first version did the
 // transpose-reduce with a 31-shuffle register butterfly: 124 instructions per group against 71 now.)
+#include <type_traits>
+
 #include "gs_common.cuh"
 
 namespace {
@@ -94,13 +96,14 @@ __device__ __forceinline__ bool pixel_grad(PixState &ps, bool live, uint32_t rec
     return true;
 }
 
-template <int DEPTH, int CB_BATCH, int MINB>
+// ALPHA: dL/d(accumulated opacity) per pixel joins the background term (GsAlpha; false is the kernel of before)
+template <int DEPTH, int CB_BATCH, int MINB, bool ALPHA = false>
 __global__ void __launch_bounds__(CB_THREADS, MINB)
 k_composite_bwd_v1(const DevCfg c, const float4 *__restrict__ rec0, const float4 *__restrict__ rec1,
                 const float4 *__restrict__ rec2, const uint32_t *__restrict__ point_list,
                 const uint2 *__restrict__ ranges, const float *__restrict__ final_T,
                 const uint32_t *__restrict__ n_contrib, const float *__restrict__ dL_dcolor,
-                const float *__restrict__ dL_ddepth, float *__restrict__ acc) {
+                const float *__restrict__ dL_ddepth, float *__restrict__ acc, const float *__restrict__ dL_dalpha) {
     // double-buffered staging, as in the forward: the cp.async gathers of the next batch land in one buffer while the
     // warps walk the other
     extern __shared__ __align__(16) unsigned char cb_smem[];
@@ -148,6 +151,8 @@ k_composite_bwd_v1(const DevCfg c, const float4 *__restrict__ rec0, const float4
     for (int ch = 0; ch < 3; ch++) ps.accum[ch] = ps.last_color[ch] = 0.f;
     const float *bg = c.bg ? c.bg + (size_t)v * 3 : nullptr;
     ps.bg_dot = bg ? bg[0] * ps.dLp[0] + bg[1] * ps.dLp[1] + bg[2] * ps.dLp[2] : 0.f;
+    // alpha = 1 - T_final: its gradient is the background's with dL/dalpha in place of -bg . dL/dC
+    if (ALPHA && inside) ps.bg_dot -= dL_dalpha[(size_t)v * hw + pix];
 
     // the walk starts at the deepest position any pixel of the tile reached
     const uint32_t warp_last = __reduce_max_sync(0xffffffffu, ps.last);
@@ -288,15 +293,17 @@ struct Cb2Smem {
 // instead of float REDs, so the totals do not depend on the order in which warps arrive.  A term with no encoding
 // (non-finite, out of range) sets its component's bit in the poison mask.  DET = false is the default kernel,
 // instruction for instruction (the two trailing parameters are unused).  DEPTH: as k_composite_fwd (2: the depth term of
-// dL/dalpha takes rec2.w).
-template <int DEPTH, int CB_BATCH, int MINB, bool DET = false>
+// dL/dalpha takes rec2.w).  ALPHA: dL/d(accumulated opacity) per pixel joins the background term Y (GsAlpha; false is the
+// kernel of before, instruction for instruction).
+template <int DEPTH, int CB_BATCH, int MINB, bool DET = false, bool ALPHA = false>
 __global__ void __launch_bounds__(CB_THREADS, MINB)
 k_composite_bwd(const DevCfg c, const float4 *__restrict__ rec0, const float4 *__restrict__ rec1,
                 const float4 *__restrict__ rec2, const uint32_t *__restrict__ point_list,
                 const uint2 *__restrict__ ranges, const float *__restrict__ final_T,
                 const uint32_t *__restrict__ n_contrib, const float *__restrict__ dL_dcolor,
                 const float *__restrict__ dL_ddepth, float *__restrict__ acc,
-                unsigned long long *__restrict__ det_acc, uint32_t *__restrict__ det_poison) {
+                unsigned long long *__restrict__ det_acc, uint32_t *__restrict__ det_poison,
+                const float *__restrict__ dL_dalpha) {
     extern __shared__ __align__(16) unsigned char cb_smem[];
     Cb2Smem<CB_BATCH> &sm = *reinterpret_cast<Cb2Smem<CB_BATCH> *>(cb_smem);
     auto &s_rec = sm.rec;
@@ -332,7 +339,11 @@ k_composite_bwd(const DevCfg c, const float4 *__restrict__ rec0, const float4 *_
         dl.z = dlp[2 * hw];
         if (DEPTH && dL_ddepth) dl.w = dL_ddepth[(size_t)v * hw + pix];
         const float *bg = c.bg ? c.bg + (size_t)v * 3 : nullptr;
-        if (bg) Y = T * (bg[0] * dl.x + bg[1] * dl.y + bg[2] * dl.z);   // the background term of every dL/dalpha
+        if constexpr (ALPHA) {
+            // alpha = 1 - T_final enters exactly as the background does, with dL/dalpha in place of -bg . dL/dC
+            const float bg_dot = bg ? bg[0] * dl.x + bg[1] * dl.y + bg[2] * dl.z : 0.f;
+            Y = T * (bg_dot - dL_dalpha[(size_t)v * hw + pix]);
+        } else if (bg) Y = T * (bg[0] * dl.x + bg[1] * dl.y + bg[2] * dl.z);   // the background term of every dL/dalpha
     }
     sm.dl[warp][lane] = dl;
 
@@ -517,7 +528,7 @@ k_composite_bwd(const DevCfg c, const float4 *__restrict__ rec0, const float4 *_
 }  // namespace
 
 int launch_composite_bwd(const DevCfg &c, const GsSaved &s, const float *dL_dcolor, const float *dL_ddepth,
-                         float *grad_acc, cudaStream_t st, int variant, const DetAcc &det) {
+                         float *grad_acc, cudaStream_t st, int variant, const DetAcc &det, const float *dL_dalpha) {
     if (c.V == 0 || c.ntiles == 0) return GS_OK;
     dim3 grid(c.ntiles, c.V);
     if (variant != 1) {
@@ -527,25 +538,28 @@ int launch_composite_bwd(const DevCfg &c, const GsSaved &s, const float *dL_dcol
         auto launch = [&](auto kern, size_t smem) -> int {
             GS_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
             kern<<<grid, CB_THREADS, smem, st>>>(c, s.rec0, s.rec1, s.rec2, s.point_list, s.ranges, s.final_T, s.n_contrib,
-                                                 dL_dcolor, dL_ddepth, grad_acc, det.acc, det.poison);
+                                                 dL_dcolor, dL_ddepth, grad_acc, det.acc, det.poison, dL_dalpha);
             return GS_OK;
         };
         const bool dep = (c.flags & GS_FLAG_DEPTH) != 0;
-        int rc;
-        if (dep && s.depth_mode != GS_DEPTH_Z) {   // the depth channel carried f(z) in rec2.w
-            if (det.acc)
-                rc = variant == 2 ? launch(k_composite_bwd<2, 128, 4, true>, sizeof(Cb2Smem<128>)) : launch(k_composite_bwd<2, 256, 3, true>, sizeof(Cb2Smem<256>));
-            else
-                rc = variant == 2 ? launch(k_composite_bwd<2, 128, 4>, sizeof(Cb2Smem<128>)) : launch(k_composite_bwd<2, 256, 3>, sizeof(Cb2Smem<256>));
-        } else if (det.acc) {
+        // A: an incoming alpha gradient (the ALPHA instantiations); without one, the kernels of before
+        auto pick = [&](auto alpha_tag) -> int {
+            constexpr bool A = decltype(alpha_tag)::value;
+            if (dep && s.depth_mode != GS_DEPTH_Z) {   // the depth channel carried f(z) in rec2.w
+                if (det.acc)
+                    return variant == 2 ? launch(k_composite_bwd<2, 128, 4, true, A>, sizeof(Cb2Smem<128>)) : launch(k_composite_bwd<2, 256, 3, true, A>, sizeof(Cb2Smem<256>));
+                return variant == 2 ? launch(k_composite_bwd<2, 128, 4, false, A>, sizeof(Cb2Smem<128>)) : launch(k_composite_bwd<2, 256, 3, false, A>, sizeof(Cb2Smem<256>));
+            }
+            if (det.acc) {
+                if (variant == 2)
+                    return dep ? launch(k_composite_bwd<1, 128, 4, true, A>, sizeof(Cb2Smem<128>)) : launch(k_composite_bwd<0, 128, 4, true, A>, sizeof(Cb2Smem<128>));
+                return dep ? launch(k_composite_bwd<1, 256, 3, true, A>, sizeof(Cb2Smem<256>)) : launch(k_composite_bwd<0, 256, 3, true, A>, sizeof(Cb2Smem<256>));
+            }
             if (variant == 2)
-                rc = dep ? launch(k_composite_bwd<1, 128, 4, true>, sizeof(Cb2Smem<128>)) : launch(k_composite_bwd<0, 128, 4, true>, sizeof(Cb2Smem<128>));
-            else
-                rc = dep ? launch(k_composite_bwd<1, 256, 3, true>, sizeof(Cb2Smem<256>)) : launch(k_composite_bwd<0, 256, 3, true>, sizeof(Cb2Smem<256>));
-        } else if (variant == 2)
-            rc = dep ? launch(k_composite_bwd<1, 128, 4>, sizeof(Cb2Smem<128>)) : launch(k_composite_bwd<0, 128, 4>, sizeof(Cb2Smem<128>));
-        else
-            rc = dep ? launch(k_composite_bwd<1, 256, 3>, sizeof(Cb2Smem<256>)) : launch(k_composite_bwd<0, 256, 3>, sizeof(Cb2Smem<256>));
+                return dep ? launch(k_composite_bwd<1, 128, 4, false, A>, sizeof(Cb2Smem<128>)) : launch(k_composite_bwd<0, 128, 4, false, A>, sizeof(Cb2Smem<128>));
+            return dep ? launch(k_composite_bwd<1, 256, 3, false, A>, sizeof(Cb2Smem<256>)) : launch(k_composite_bwd<0, 256, 3, false, A>, sizeof(Cb2Smem<256>));
+        };
+        const int rc = dL_dalpha ? pick(std::true_type{}) : pick(std::false_type{});
         if (rc != GS_OK) return rc;
         GS_CUDA_OK(cudaGetLastError());
         return GS_OK;
@@ -558,10 +572,13 @@ int launch_composite_bwd(const DevCfg &c, const GsSaved &s, const float *dL_dcol
     auto launch = [&](auto kern) -> int {
         GS_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         kern<<<grid, CB_THREADS, smem, st>>>(c, s.rec0, s.rec1, s.rec2, s.point_list, s.ranges, s.final_T, s.n_contrib,
-                                             dL_dcolor, dL_ddepth, grad_acc);
+                                             dL_dcolor, dL_ddepth, grad_acc, dL_dalpha);
         return GS_OK;
     };
-    const int rc = !(c.flags & GS_FLAG_DEPTH) ? launch(k_composite_bwd_v1<0, BATCH, MINB>)
+    const int rc = dL_dalpha ? (!(c.flags & GS_FLAG_DEPTH) ? launch(k_composite_bwd_v1<0, BATCH, MINB, true>)
+                                : s.depth_mode == GS_DEPTH_Z ? launch(k_composite_bwd_v1<1, BATCH, MINB, true>)
+                                                              : launch(k_composite_bwd_v1<2, BATCH, MINB, true>))
+                   : !(c.flags & GS_FLAG_DEPTH) ? launch(k_composite_bwd_v1<0, BATCH, MINB>)
                    : s.depth_mode == GS_DEPTH_Z ? launch(k_composite_bwd_v1<1, BATCH, MINB>)
                                                  : launch(k_composite_bwd_v1<2, BATCH, MINB>);
     if (rc != GS_OK) return rc;

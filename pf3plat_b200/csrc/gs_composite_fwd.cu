@@ -35,12 +35,13 @@ struct CfStage {
 
 // DEPTH: 0 no depth channel; 1 the channel composites rec2.y (GS_DEPTH_Z); 2 it composites rec2.w, the f(z) preprocess
 // stored for the other depth modes.  Values 0 and 1 are the kernels of before, instruction for instruction.
-template <int DEPTH, int MINB>
+// ALPHA: also store the accumulated opacity 1 - T next to final_T (GsAlpha); false is the kernel of before.
+template <int DEPTH, int MINB, bool ALPHA = false>
 __global__ void __launch_bounds__(CF_THREADS, MINB)
 k_composite_fwd(const DevCfg c, const float4 *__restrict__ rec0, const float4 *__restrict__ rec1,
                 const float4 *__restrict__ rec2, const uint32_t *__restrict__ point_list,
                 const uint2 *__restrict__ ranges, float *__restrict__ color, float *__restrict__ depth,
-                float *__restrict__ final_T, uint32_t *__restrict__ n_contrib) {
+                float *__restrict__ final_T, uint32_t *__restrict__ n_contrib, float *__restrict__ alpha_out) {
     __shared__ CfStage stage[2];
 
     const int v = blockIdx.y;
@@ -147,6 +148,7 @@ k_composite_fwd(const DevCfg c, const float4 *__restrict__ rec0, const float4 *_
         out[2 * hw] = C2 + T * (bg ? bg[2] : 0.f);
         if (DEPTH) depth[(size_t)v * hw + pix] = Dz;
         final_T[(size_t)v * hw + pix] = T;
+        if (ALPHA) alpha_out[(size_t)v * hw + pix] = 1.0f - T;
         n_contrib[(size_t)v * hw + pix] = last;
     }
 }
@@ -190,13 +192,13 @@ __device__ __forceinline__ uint32_t ld_volatile_shared(const uint32_t *p) {
     return v;
 }
 
-template <int DEPTH, int MINB>   // DEPTH as k_composite_fwd
+template <int DEPTH, int MINB, bool ALPHA = false>   // DEPTH, ALPHA as k_composite_fwd
 __global__ void __launch_bounds__(CP_THREADS, MINB)
 k_composite_fwd_ws(const DevCfg c, const float4 *__restrict__ rec0, const float4 *__restrict__ rec1,
                    const float4 *__restrict__ rec2, const uint32_t *__restrict__ point_list,
                    const uint2 *__restrict__ ranges, float *__restrict__ color, float *__restrict__ depth,
                    float *__restrict__ final_T, uint32_t *__restrict__ n_contrib, uint32_t *__restrict__ sched,
-                const uint32_t total_tiles) {
+                const uint32_t total_tiles, float *__restrict__ alpha_out) {
     __shared__ __align__(16) CpSmem sm;
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     if (tid == 0) {
@@ -343,6 +345,7 @@ k_composite_fwd_ws(const DevCfg c, const float4 *__restrict__ rec0, const float4
             out[2 * hw] = C2 + T * (bg ? bg[2] : 0.f);
             if (DEPTH) depth[(size_t)v * hw + pix] = Dz;
             final_T[(size_t)v * hw + pix] = T;
+            if (ALPHA) alpha_out[(size_t)v * hw + pix] = 1.0f - T;
             n_contrib[(size_t)v * hw + pix] = last;
         }
     }
@@ -350,7 +353,8 @@ k_composite_fwd_ws(const DevCfg c, const float4 *__restrict__ rec0, const float4
 
 }  // namespace
 
-int launch_composite_fwd(const DevCfg &c, const GsSaved &s, float *color, float *depth, cudaStream_t st, int variant) {
+int launch_composite_fwd(const DevCfg &c, const GsSaved &s, float *color, float *depth, cudaStream_t st, int variant,
+                         float *alpha) {
     if (c.V == 0 || c.ntiles == 0) return GS_OK;
     if (variant == 2) {
         // warp-specialised variant: persistent grid of SMs x resident CTAs; tiles handed out through s.sched
@@ -371,9 +375,13 @@ int launch_composite_fwd(const DevCfg &c, const GsSaved &s, float *color, float 
         GS_CUDA_OK(cudaMemsetAsync(s.sched, 0, 8, st));
         auto launch_ws = [&](auto kern) {
             kern<<<nctas, CP_THREADS, 0, st>>>(c, s.rec0, s.rec1, s.rec2, s.point_list, s.ranges, color, depth, s.final_T,
-                                               s.n_contrib, s.sched, total);
+                                               s.n_contrib, s.sched, total, alpha);
         };
-        if (depth_kind == 2) launch_ws(k_composite_fwd_ws<2, MINB_WS>);
+        if (alpha) {
+            if (depth_kind == 2) launch_ws(k_composite_fwd_ws<2, MINB_WS, true>);
+            else if (depth_kind == 1) launch_ws(k_composite_fwd_ws<1, MINB_WS, true>);
+            else launch_ws(k_composite_fwd_ws<0, MINB_WS, true>);
+        } else if (depth_kind == 2) launch_ws(k_composite_fwd_ws<2, MINB_WS>);
         else if (depth_kind == 1) launch_ws(k_composite_fwd_ws<1, MINB_WS>);
         else launch_ws(k_composite_fwd_ws<0, MINB_WS>);
         GS_CUDA_OK(cudaGetLastError());
@@ -384,9 +392,14 @@ int launch_composite_fwd(const DevCfg &c, const GsSaved &s, float *color, float 
     // C2 -- issue-bound, like the backward.
     constexpr int MINB = 6;
     auto launch = [&](auto kern) {
-        kern<<<grid, CF_THREADS, 0, st>>>(c, s.rec0, s.rec1, s.rec2, s.point_list, s.ranges, color, depth, s.final_T, s.n_contrib);
+        kern<<<grid, CF_THREADS, 0, st>>>(c, s.rec0, s.rec1, s.rec2, s.point_list, s.ranges, color, depth, s.final_T, s.n_contrib,
+                                          alpha);
     };
-    if (!(c.flags & GS_FLAG_DEPTH)) launch(k_composite_fwd<0, MINB>);
+    if (alpha) {
+        if (!(c.flags & GS_FLAG_DEPTH)) launch(k_composite_fwd<0, MINB, true>);
+        else if (s.depth_mode == GS_DEPTH_Z) launch(k_composite_fwd<1, MINB, true>);
+        else launch(k_composite_fwd<2, MINB, true>);
+    } else if (!(c.flags & GS_FLAG_DEPTH)) launch(k_composite_fwd<0, MINB>);
     else if (s.depth_mode == GS_DEPTH_Z) launch(k_composite_fwd<1, MINB>);
     else launch(k_composite_fwd<2, MINB>);
     GS_CUDA_OK(cudaGetLastError());

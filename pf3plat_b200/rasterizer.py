@@ -172,6 +172,9 @@ class BatchSettings(NamedTuple):
     # view-scaled scene), "disparity", "relative_disparity" or "log" (f(z) of render_depth_cuda at the unscaled z)
     depth_mode: str = "depth"
     depth_near_far: Optional[torch.Tensor] = None  # (V,2) unscaled near, far: needed by "relative_disparity" and "log"
+    # also return the accumulated opacity alpha = 1 - T_final (V,H,W) of the colour pass (GsAlpha); its gradient reaches
+    # the geometry and the opacities, never SH, colours or cameras
+    with_alpha: bool = False
 
 
 # ---------------------------------------------------------------------------------------------------------
@@ -243,7 +246,8 @@ class _RasterizeBatch(torch.autograd.Function):
     one only through the fused depth channel (bs.with_depth), as the reference's depth pass gives its cameras one
     through its fake colour z (cuda_splatting.py:239-242): dL/dviewmatrix is zero outside the z column, and None when
     the depth is not part of the loss.  Colour, projection and culling give the cameras no gradient, as in the
-    reference op.  Under torch.use_deterministic_algorithms(True) the backward is bit-reproducible."""
+    reference op.  bs.with_alpha appends the accumulated opacity (gs_forward_ex / gs_backward_ex); it gives the cameras
+    no gradient either.  Under torch.use_deterministic_algorithms(True) the backward is bit-reproducible."""
 
     @staticmethod
     def forward(ctx, means3D, means2D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp, viewmatrix,
@@ -275,14 +279,20 @@ class _RasterizeBatch(torch.autograd.Function):
             radii = torch.empty((V, P), dtype=torch.int32, device=dev)
             depth = torch.empty((V, H, W), dtype=torch.float32, device=dev) if bs.with_depth else None
             gout = GsOutputs(_ptr(color), _ptr(radii), _ptr(depth))
+            alpha = torch.empty((V, H, W), dtype=torch.float32, device=dev) if bs.with_alpha else None
             want_view_z = bs.with_depth and viewmatrix.requires_grad
             needs_grad = want_view_z or any(t is not None and t.requires_grad for t in
                                             (means3D, means2D, shs, colors_precomp, opacities, scales, rotations,
                                              cov3D_precomp))
             saved = ctypes.c_void_p()
             with _context_lock(dev, stream_ptr):
-                rc = _capi.lib().gs_forward(gctx, ctypes.byref(cfg), ctypes.byref(gin), ctypes.byref(gout),
-                                            ctypes.byref(saved) if needs_grad else None, stream_ptr)
+                if alpha is not None:
+                    rc = _capi.lib().gs_forward_ex(gctx, ctypes.byref(cfg), ctypes.byref(gin), ctypes.byref(gout),
+                                                   ctypes.byref(_capi.GsAlpha(_ptr(alpha), None)),
+                                                   ctypes.byref(saved) if needs_grad else None, stream_ptr)
+                else:
+                    rc = _capi.lib().gs_forward(gctx, ctypes.byref(cfg), ctypes.byref(gin), ctypes.byref(gout),
+                                                ctypes.byref(saved) if needs_grad else None, stream_ptr)
                 _capi.check(rc)
         if needs_grad:
             ctx.handle = _SavedHandle(gctx, saved, stream_ptr, dev)
@@ -299,12 +309,10 @@ class _RasterizeBatch(torch.autograd.Function):
             ctx.want_means2D = means2D is not None and means2D.requires_grad
             ctx.view_z = (viewmatrix.shape, viewmatrix.dtype) if want_view_z else None
         ctx.mark_non_differentiable(radii)
-        if bs.with_depth:
-            return color, radii, depth
-        return color, radii
+        return (color, radii) + ((depth,) if bs.with_depth else ()) + ((alpha,) if bs.with_alpha else ())
 
     @staticmethod
-    def backward(ctx, grad_color, grad_radii=None, grad_depth=None):
+    def backward(ctx, grad_color, grad_radii=None, *grad_extra):
         S, P, V, M, H, W = ctx.dims
         ins = ctx.ins
         for name, t, version in ctx.versions:
@@ -313,6 +321,9 @@ class _RasterizeBatch(torch.autograd.Function):
                                    f"operation: {name} is at version {t._version}; expected version {version} instead")
         dev = ins["means3D"].device
         bs = ctx.bs
+        grad_depth = grad_extra[0] if bs.with_depth else None
+        # an alpha the loss does not read arrives as None: the call is then gs_backward's, kernels included
+        grad_alpha = grad_extra[-1] if bs.with_alpha else None
         keep: list = []
         with torch.cuda.device(dev):
             stream_ptr = torch.cuda.current_stream(dev).cuda_stream
@@ -338,8 +349,14 @@ class _RasterizeBatch(torch.autograd.Function):
             }
             ig = GsInGrads(**{k: _ptr(t) for k, t in g.items()})
             with _context_lock(dev, stream_ptr):
-                rc = _capi.lib().gs_backward(gctx, ctypes.byref(cfg), ctypes.byref(gin), ctx.handle.ptr, ctypes.byref(og),
-                                             ctypes.byref(ig), stream_ptr)
+                if grad_alpha is not None:
+                    galpha = _f32c(grad_alpha)
+                    rc = _capi.lib().gs_backward_ex(gctx, ctypes.byref(cfg), ctypes.byref(gin), ctx.handle.ptr,
+                                                    ctypes.byref(og), ctypes.byref(_capi.GsAlpha(None, _ptr(galpha))),
+                                                    ctypes.byref(ig), stream_ptr)
+                else:
+                    rc = _capi.lib().gs_backward(gctx, ctypes.byref(cfg), ctypes.byref(gin), ctx.handle.ptr,
+                                                 ctypes.byref(og), ctypes.byref(ig), stream_ptr)
                 _capi.check(rc)
             gview = None
             if g["dL_dviewmatrix_z"] is not None:
@@ -356,8 +373,9 @@ def rasterize_batch(bs: BatchSettings, means3D, opacities, shs=None, colors_prec
                     rotations=None, cov3D_precomp=None, means2D=None):
     """Batched operator.  Shapes: means3D (S,P,3); opacities (S,P) or (S,P,1); shs (S,P,M,3); colors_precomp
     (V,P,3); scales (S,P,3); rotations (S,P,4); cov3D_precomp (S,P,6); means2D (V,P,3) (gradient sink only).
-    Returns (color (V,3,H,W), radii (V,P)[, depth (V,H,W)]).  With bs.with_depth, a bs.viewmatrix that requires grad
-    gets dL/ddepth's gradient in its z column (see _RasterizeBatch)."""
+    Returns (color (V,3,H,W), radii (V,P)[, depth (V,H,W)][, alpha (V,H,W)]).  With bs.with_depth, a bs.viewmatrix that
+    requires grad gets dL/ddepth's gradient in its z column (see _RasterizeBatch); bs.with_alpha appends the accumulated
+    opacity 1 - T_final."""
     _check_exclusive(shs, colors_precomp, scales, rotations, cov3D_precomp)
     # means2D exists in the reference op only as a sink for the screen-space gradient (cuda_splatting.py:93-97); the
     # batched entry neither allocates nor fills it unless the caller passes one
@@ -409,14 +427,13 @@ class GaussianRasterizer(nn.Module):
             return present.bool()
 
     def forward(self, means3D, means2D, opacities, shs=None, colors_precomp=None, scales=None, rotations=None,
-                cov3D_precomp=None, return_depth: bool = False):
+                cov3D_precomp=None, return_depth: bool = False, return_alpha: bool = False):
         """Returns (color (3,H,W), radii (P,)) like the reference op; `return_depth=True` (opt-in, not used by
-        PF3plat) appends the composited camera-space depth (H,W)."""
+        PF3plat) appends the composited camera-space depth (H,W), `return_alpha=True` then the accumulated opacity
+        1 - T_final (H,W)."""
         _check_exclusive(shs, colors_precomp, scales, rotations, cov3D_precomp)
         u = lambda t: None if t is None else t.unsqueeze(0)
-        bs = self._batch_settings(means3D.device, with_depth=return_depth)
+        bs = self._batch_settings(means3D.device, with_depth=return_depth)._replace(with_alpha=bool(return_alpha))
         out = _RasterizeBatch.apply(u(means3D), u(means2D), u(shs), u(colors_precomp), u(opacities), u(scales),
                                     u(rotations), u(cov3D_precomp), bs.viewmatrix, bs)
-        if return_depth:
-            return out[0][0], out[1][0], out[2][0]
-        return out[0][0], out[1][0]
+        return tuple(o[0] for o in out)

@@ -33,7 +33,7 @@ def _cov6(cov: torch.Tensor) -> torch.Tensor:
 def render_views(extrinsics, intrinsics, near, far, image_shape, background_color, gaussian_means,
                  gaussian_covariances, gaussian_sh_coefficients, gaussian_opacities, scale_invariant: bool = True,
                  use_sh: bool = True, with_depth: bool = False, sh_layout: str = "g_xyz_n",
-                 sh_eval_max_degree: Optional[int] = None, depth_mode: str = "depth"):
+                 sh_eval_max_degree: Optional[int] = None, depth_mode: str = "depth", with_alpha: bool = False):
     """extrinsics (B,4,4) c2w, intrinsics (B,3,3), near/far (B,), background (B,3); Gaussians are per SCENE and NOT
     repeated per view: means (S,G,3), covariances (S,G,3,3) or (S,G,6), sh (S,G,3,d_sh) [or (S,G,d_sh,3) with
     sh_layout="g_n_xyz"], opacities (S,G); B % S == 0 and view b shows scene b // (B//S).
@@ -41,7 +41,8 @@ def render_views(extrinsics, intrinsics, near, far, image_shape, background_colo
     (rasterizer.set_sh_eval_max_degree, default 3).
     Returns color (B,3,h,w) and, if with_depth, depth (B,h,w) = sum_i alpha_i T_i f(z_i): f(z) = z of the (rescaled)
     scene for depth_mode "depth"; for "disparity", "relative_disparity" and "log" the fake colour of render_depth_cuda
-    (cuda_splatting.py:245-251) at the UNSCALED camera-space depth z, with the unscaled near and far."""
+    (cuda_splatting.py:245-251) at the UNSCALED camera-space depth z, with the unscaled near and far.
+    with_alpha: also return the accumulated opacity alpha (B,h,w) = 1 - T_final, last: (color[, depth], alpha)."""
     assert use_sh or gaussian_sh_coefficients.shape[-1 if sh_layout == "g_xyz_n" else -2] == 1
     h, w = image_shape
     vb = make_view_batch(extrinsics, intrinsics, near, far, scale_invariant)
@@ -58,7 +59,8 @@ def render_views(extrinsics, intrinsics, near, far, image_shape, background_colo
                        campos=vb.campos, bg=background_color, sh_degree=degree, tanfov=vb.tanfov,
                        view_scale=vb.scale if scale_invariant else None, with_depth=with_depth,
                        sh_eval_max_degree=sh_eval_max_degree, depth_mode=depth_mode,
-                       depth_near_far=torch.stack([near, far], -1) if with_depth and depth_mode != "depth" else None)
+                       depth_near_far=torch.stack([near, far], -1) if with_depth and depth_mode != "depth" else None,
+                       with_alpha=with_alpha)
     B = extrinsics.shape[0]
     S = gaussian_means.shape[0]
     if use_sh:
@@ -67,6 +69,8 @@ def render_views(extrinsics, intrinsics, near, far, image_shape, background_colo
         colors = shs[..., 0, :]                                  # (S,G,3)
         colors = colors.repeat_interleave(B // S, dim=0) if S != B else colors
         out = rasterize_batch(bs, gaussian_means, gaussian_opacities, colors_precomp=colors, cov3D_precomp=cov6)
+    if with_alpha:
+        return (out[0], out[2], out[3]) if with_depth else (out[0], out[2])
     if with_depth:
         return out[0], out[2]
     return out[0]
@@ -81,7 +85,8 @@ def render_cuda(extrinsics, intrinsics, near, far, image_shape, background_color
 
 
 def decoder_forward(means, covariances, harmonics, opacities, extrinsics, intrinsics, near, far, image_shape,
-                    background_color, depth_mode: Optional[str] = None, sh_eval_max_degree: Optional[int] = None):
+                    background_color, depth_mode: Optional[str] = None, sh_eval_max_degree: Optional[int] = None,
+                    return_alpha: bool = False):
     """`DecoderSplattingCUDA.forward` (decoder_splatting_cuda.py:35-67) without the v-fold repeat: Gaussians
     (b,g,...), cameras (b,v,...).  Returns (color (b,v,3,h,w), depth (b,v,h,w) or None).  Every depth_mode of the
     reference ("depth", "disparity", "relative_disparity", "log") is composited in the same pass as the colour.
@@ -93,22 +98,31 @@ def decoder_forward(means, covariances, harmonics, opacities, extrinsics, intrin
     mode's f'(z) (make_view_batch carries it on to the extrinsics), besides the Gaussians.  "log" clamps z as the
     reference does, to the constant log(far) when near < far: its extrinsics get a zero gradient.  A loss that does not
     read the depth leaves the extrinsics without a gradient, as the reference does.  So every mode is one render whether
-    or not the extrinsics require grad.  sh_eval_max_degree: as render_views."""
+    or not the extrinsics require grad.  sh_eval_max_degree: as render_views.
+    return_alpha: also return the accumulated opacity (b,v,h,w) = 1 - T_final of the same pass, as (color, depth, alpha)
+    (depth None without a depth_mode).  It trains the Gaussians' geometry and opacities, never the extrinsics."""
     b, v = extrinsics.shape[:2]
     flat = lambda t: t.reshape(b * v, *t.shape[2:])
     bg = background_color.reshape(1, 3).expand(b * v, 3)
     out = render_views(flat(extrinsics), flat(intrinsics), flat(near), flat(far), image_shape, bg, means,
                        covariances, harmonics, opacities, with_depth=depth_mode is not None,
-                       sh_eval_max_degree=sh_eval_max_degree, depth_mode=depth_mode or "depth")
+                       sh_eval_max_degree=sh_eval_max_degree, depth_mode=depth_mode or "depth", with_alpha=return_alpha)
+    alpha = None
+    if return_alpha:
+        *out, alpha = out
+        out = out[0] if depth_mode is None else tuple(out)
+        alpha = alpha.reshape(b, v, *alpha.shape[1:])
     if depth_mode is None:
-        return out.reshape(b, v, *out.shape[1:]), None
+        color = out.reshape(b, v, *out.shape[1:])
+        return (color, None, alpha) if return_alpha else (color, None)
     color, depth = out
     if depth_mode == "depth":
         # the reference renders depth in the 1/near-rescaled scene (render_depth_cuda -> render_cuda with
         # scale_invariant=True) but takes the fake colour from the UNSCALED camera-space z
         # (cuda_splatting.py:239-242): undo the rescale of z (the other modes evaluate f at the unscaled z already)
         depth = depth * flat(near)[:, None, None]
-    return color.reshape(b, v, *color.shape[1:]), depth.reshape(b, v, *depth.shape[1:])
+    color, depth = color.reshape(b, v, *color.shape[1:]), depth.reshape(b, v, *depth.shape[1:])
+    return (color, depth, alpha) if return_alpha else (color, depth)
 
 
 def render_depth(means, covariances, opacities, extrinsics, intrinsics, near, far, image_shape, mode: str = "depth"):

@@ -59,7 +59,17 @@ enum {
      * component NaN) instead of float atomics, and the view-matrix gradient is summed in a fixed order.  Needs
      * 244 B instead of 40 B of context scratch per (view, Gaussian); frames with ceil(H/4) * ceil(W/8) >= 2^21 and
      * GS_TUNE_BWD_V1 are rejected (GS_ERR_INVALID).  The forward ignores it: it is deterministic already. */
-    GS_FLAG_DETERMINISTIC = 4u
+    GS_FLAG_DETERMINISTIC = 4u,
+    /* Anti-aliasing: the screen-space filter with opacity compensation (Mip-Splatting's 2-D filter, upstream's
+     * `antialiasing` setting).  Per (view, Gaussian), with (a0, b, c0) the projected 2-D covariance before the dilation
+     * h = GsConfig::dilation, the splat is drawn with the dilated covariance (a0 + h, b, c0 + h), as always, but at opacity
+     * o * rho, rho = sqrt(max(2.5e-5, (a0 c0 - b^2) / ((a0 + h)(c0 + h) - b^2))): a sub-pixel splat keeps the weight of
+     * its own footprint instead of covering the dilated one at full opacity.  Tile binning uses o * rho.  The backward
+     * differentiates rho into opacities, covariances or scales / rotations and means (not the cameras); it follows its
+     * forward's setting, whatever its own flags say.  GS_TUNE_PRE_OCC6 and GS_TUNE_PBWD_2PHASE have no anti-aliased
+     * kernels: with this flag they are GS_ERR_INVALID.  Libraries that predate it ignore the bit: see
+     * gs_supported_flags(). */
+    GS_FLAG_ANTIALIAS = 8u
 };
 
 enum {
@@ -202,6 +212,9 @@ typedef struct GsSaved GsSaved;     /* state a forward keeps for its backward (w
 
 GS_API int gs_abi_version(void);
 GS_API const char *gs_last_error(void);
+/* The GS_FLAG_* bits this library honours (unknown bits of GsConfig::flags are ignored, not refused): a host checks it
+ * before it relies on a flag that a library of the same ABI version may predate, such as GS_FLAG_ANTIALIAS. */
+GS_API uint32_t gs_supported_flags(void);
 
 /* Workspace lifetime (upstream allocates scratch through torch callbacks on every call; here it is a grow-only cache). */
 GS_API int gs_context_create(GsContext **out);

@@ -17,6 +17,7 @@ ABI_VERSION = 5
 GS_FLAG_DEPTH = 1
 GS_FLAG_PREFILTERED = 2
 GS_FLAG_DETERMINISTIC = 4
+GS_FLAG_ANTIALIAS = 8
 GS_DEPTH_Z = 0
 GS_DEPTH_DISPARITY = 1
 GS_DEPTH_RELATIVE_DISPARITY = 2
@@ -128,6 +129,7 @@ class GsLpipsConfig(Structure):
 SYMBOLS = {
     "gs_abi_version": (c_int, []),
     "gs_last_error": (c_char_p, []),
+    "gs_supported_flags": (c_uint32, []),
     "gs_context_create": (c_int, [POINTER(c_void_p)]),
     "gs_context_destroy": (None, [c_void_p]),
     "gs_context_trim": (c_int, [c_void_p]),

@@ -22,6 +22,9 @@ int gs_set_cuda_error(cudaError_t e, const char *what, const char *file, int lin
 
 extern "C" const char *gs_last_error(void) { return g_err; }
 extern "C" int gs_abi_version(void) { return GS_ABI_VERSION; }
+extern "C" uint32_t gs_supported_flags(void) {
+    return GS_FLAG_DEPTH | GS_FLAG_PREFILTERED | GS_FLAG_DETERMINISTIC | GS_FLAG_ANTIALIAS;
+}
 
 // ---------------------------------------------------------------------------------------------------------
 // context: grow-only scratch, pinned read-back word, optional stage timers
@@ -141,6 +144,17 @@ int validate_depth_mode(const GsConfig *cfg) {
         return gs_set_error(GS_ERR_INVALID, "depth_mode GS_DEPTH_RELATIVE_DISPARITY / GS_DEPTH_LOG needs depth_near_far");
     return GS_OK;
 }
+
+// GS_FLAG_ANTIALIAS has no kernel behind two tuning knobs (the forward refuses both: its backward could not run)
+int validate_antialias(uint32_t flags, uint32_t tuning, uint32_t knobs) {
+    if (!(flags & GS_FLAG_ANTIALIAS)) return GS_OK;
+    if (tuning & knobs & GS_TUNE_PRE_OCC6)
+        return gs_set_error(GS_ERR_INVALID, "GS_TUNE_PRE_OCC6 has no anti-aliased kernel (GS_FLAG_ANTIALIAS)");
+    if (tuning & knobs & GS_TUNE_PBWD_2PHASE)
+        return gs_set_error(GS_ERR_INVALID, "GS_TUNE_PBWD_2PHASE has no anti-aliased kernel (GS_FLAG_ANTIALIAS)");
+    return GS_OK;
+}
+constexpr uint32_t AA_FWD_KNOBS = GS_TUNE_PRE_OCC6 | GS_TUNE_PBWD_2PHASE, AA_BWD_KNOBS = GS_TUNE_PBWD_2PHASE;
 
 DevCfg make_dev_cfg(const GsConfig *cfg) {
     DevCfg c{};
@@ -563,6 +577,7 @@ int forward(GsContext *ctx, const GsConfig *cfg, const GsInputs *in, const GsOut
     if (!out->color || (cfg->P > 0 && !out->radii)) return gs_set_error(GS_ERR_INVALID, "color/radii outputs missing");
     if ((cfg->flags & GS_FLAG_DEPTH) && !out->depth) return gs_set_error(GS_ERR_INVALID, "GS_FLAG_DEPTH needs out->depth");
     if ((rc = validate_depth_mode(cfg)) != GS_OK) return rc;
+    if ((rc = validate_antialias(cfg->flags, cfg->tuning, AA_FWD_KNOBS)) != GS_OK) return rc;
     FwdCall f{};
     f.ctx = ctx; f.c = make_dev_cfg(cfg); f.di = make_dev_inputs(in); f.out = out; f.alpha = alpha; f.st = st; f.feed = feed;
     const DevCfg &c = f.c;
@@ -642,11 +657,13 @@ int backward(GsContext *ctx, const GsConfig *cfg, const GsInputs *in, const GsSa
     int rc = validate(cfg, in);
     if (rc != GS_OK) return rc;
     if (!gout->dL_dcolor) return gs_set_error(GS_ERR_INVALID, "dL_dcolor missing");
+    if ((rc = validate_antialias(cfg->flags, cfg->tuning, AA_BWD_KNOBS)) != GS_OK) return rc;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     DevCfg c = make_dev_cfg(cfg);
     if (saved->P != c.P || saved->V != c.V || saved->S != c.S || saved->H != c.H || saved->W != c.W)
         return gs_set_error(GS_ERR_INVALID, "saved state does not match the configuration");
-    c.flags = saved->flags;
+    c.flags = saved->flags;   // (GS_FLAG_ANTIALIAS included: the backward differentiates what its forward drew)
+    if ((rc = validate_antialias(c.flags, cfg->tuning, AA_BWD_KNOBS)) != GS_OK) return rc;
     if (gin->dL_dviewmatrix_z && !(c.flags & GS_FLAG_DEPTH))
         return gs_set_error(GS_ERR_INVALID, "dL_dviewmatrix_z needs a forward with GS_FLAG_DEPTH");
     // the forward's depth mode, with this call's near / far
@@ -737,6 +754,7 @@ int render_host(GsContext *ctx, const GsConfig *cfg, const GsInputs *in, const G
     int rc = validate(cfg, in);
     if (rc != GS_OK) return rc;
     if ((rc = validate_depth_mode(cfg)) != GS_OK) return rc;
+    if ((rc = validate_antialias(cfg->flags, cfg->tuning, AA_FWD_KNOBS)) != GS_OK) return rc;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     const size_t SP = (size_t)cfg->S * cfg->P, VP = (size_t)cfg->V * cfg->P, V = (size_t)cfg->V;
     const size_t px = V * cfg->image_height * cfg->image_width;

@@ -3,7 +3,7 @@
 // Data layout in HBM (DESIGN.md section 4).  Per (view, Gaussian) "splat record", three float4 SoA planes of
 // V*P entries each, written by preprocess and gathered by the compositors with 16-byte loads:
 //   rec0 = (x_pix, y_pix, -0.5*log2e*conic_a, -log2e*conic_b)
-//   rec1 = (-0.5*log2e*conic_c, opacity, r, g)
+//   rec1 = (-0.5*log2e*conic_c, opacity, r, g)   opacity: o * rho under GS_FLAG_ANTIALIAS (gs_aa_rho)
 //   rec2 = (b, z_cam, reach2, fz)     reach2 = -(log2(255*opacity) + margin): a pixel can receive the Gaussian
 //                                     only where log2 G >= reach2 (see gs_box_reaches); fz = f(z) of a depth mode
 //                                     other than GS_DEPTH_Z (the value its depth channel composites), else 0
@@ -338,6 +338,14 @@ __device__ __forceinline__ float gs_depth_chain(int mode, float zs, float s, flo
     // GS_DEPTH_LOG: d/dz log(max(min(z, near), far)) = 1/z where z passes both clamps (never, for near < far)
     return (z < near_ && z > far_) ? 1.0f / z / s : 0.0f;
 }
+
+// Anti-aliasing (GS_FLAG_ANTIALIAS, DESIGN.md 5.1): the screen-space filter's opacity compensation.  (a0, b, c0) is the
+// projected 2-D covariance before the dilation h, det1 = (a0 + h)(c0 + h) - b^2 the determinant after it; the splat is
+// drawn with the dilated covariance at opacity o * rho, rho = sqrt(max(GS_AA_RATIO_MIN, (a0 c0 - b^2) / det1)), so
+// that its footprint keeps the weight of the undilated one.  Preprocess and its backward evaluate the same expressions.
+#define GS_AA_RATIO_MIN 0.000025f
+__device__ __forceinline__ float gs_aa_ratio(float a0, float b, float c0, float det1) { return (a0 * c0 - b * b) / det1; }
+__device__ __forceinline__ float gs_aa_rho(float ratio) { return sqrtf(fmaxf(GS_AA_RATIO_MIN, ratio)); }
 
 #define GS_SH_C0 0.28209479177387814f
 #define GS_SH_C1 0.4886025119029199f

@@ -154,7 +154,9 @@ struct Splat {
 
 // Appendix A "Preprocess" for one Gaussian in one view.  COLOUR = 2: `sh` points at this Gaussian's [M][3] block in
 // shared memory; 1: `rgb_in` is its precomputed colour; 0: geometry only (the colour words are written by k_sh_colour).
-template <int COLOUR, bool B4 = false>
+// AA: GS_FLAG_ANTIALIAS -- the splat's opacity is o * rho (gs_aa_rho) wherever the kernels read it: the record and the
+// tight-binning threshold.  Conic, radius and tile rectangle stay those of the dilated covariance.
+template <int COLOUR, bool B4 = false, bool AA = false>
 __device__ __forceinline__ void project_splat(const DevCfg &c, const ViewCam &cam, float3 mean, const float *c6,
                                               float opac, const float *sh, const float *rgb_in, Splat &out) {
     out.radius = 0;
@@ -177,6 +179,11 @@ __device__ __forceinline__ void project_splat(const DevCfg &c, const ViewCam &ca
     const float cc = j.m1[0] * s1[0] + j.m1[1] * s1[1] + j.m1[2] * s1[2] + c.dilation;
     const float det = a * cc - b * b;
     if (det == 0.0f) return;
+    if constexpr (AA) {   // (the undilated diagonal: the sums above without + c.dilation)
+        const float a0 = j.m0[0] * s0[0] + j.m0[1] * s0[1] + j.m0[2] * s0[2];
+        const float c0 = j.m1[0] * s1[0] + j.m1[1] * s1[1] + j.m1[2] * s1[2];
+        opac = opac * gs_aa_rho(gs_aa_ratio(a0, b, c0, det));
+    }
     const float det_inv = 1.0f / det;
     const float A = cc * det_inv, B = -b * det_inv, C = a * det_inv;
     const float mid = 0.5f * (a + cc);
@@ -218,7 +225,8 @@ __device__ __forceinline__ void project_splat(const DevCfg &c, const ViewCam &ca
 // B4: degree-4 evaluation (25 coefficients staged per Gaussian); the B4 = false kernels are the degree-<=3 ones unchanged.
 // FZ: a depth mode other than GS_DEPTH_Z -- rec2.w = f(z) of dm.mode (a uniform runtime branch), with the views' near and
 // far staged next to their cameras.  The FZ = false kernels are the ones without it, instruction for instruction (dm unused).
-template <int COLOUR, int MINB, bool B4 = false, bool FZ = false>
+// AA: GS_FLAG_ANTIALIAS (project_splat); the AA = false kernels are the ones without it, instruction for instruction.
+template <int COLOUR, int MINB, bool B4 = false, bool FZ = false, bool AA = false>
 __global__ void __launch_bounds__(PRE_THREADS, MINB)
 k_preprocess(const DevCfg c, const DevInputs in, float4 *__restrict__ rec0, float4 *__restrict__ rec1,
              float4 *__restrict__ rec2, uint8_t *__restrict__ meta, int32_t *__restrict__ radii,
@@ -365,7 +373,7 @@ k_preprocess(const DevCfg c, const DevInputs in, float4 *__restrict__ rec0, floa
             const int v = scene * c.VPS + v0 + vi;
             const size_t o = (size_t)v * c.P + i;
             Splat sp;
-            project_splat<COLOUR, B4>(c, sm->cams[vi], mean, c6, opac, sh_s + (size_t)tid * RS,
+            project_splat<COLOUR, B4, AA>(c, sm->cams[vi], mean, c6, opac, sh_s + (size_t)tid * RS,
                                   COLOUR == 1 ? in.colors_precomp + o * 3 : nullptr, sp);
             // the depth channel's value: f at the unscaled depth z = z_s / s
             if (FZ && sp.radius > 0)
@@ -583,8 +591,18 @@ int launch_preprocess(const DevCfg &c, const DevInputs &in, float4 *rec0, float4
         kern<<<grid, PRE_THREADS, smem, st>>>(c, in, rec0, rec1, rec2, meta, radii, rects, emit, g_begin, g_end, sh_raw16, dm);
         return GS_OK;
     };
+    // anti-aliasing: the AA kernels, at 5 CTAs per SM only
+    const bool aa = (c.flags & GS_FLAG_ANTIALIAS) != 0;
+    if (aa && more_ctas)
+        return gs_set_error(GS_ERR_INVALID, "GS_TUNE_PRE_OCC6 has no anti-aliased kernel (GS_FLAG_ANTIALIAS)");
     int rc;
-    if (dm.mode != GS_DEPTH_Z) {   // rec2.w = f(z): the FZ kernels
+    if (aa) {
+        const bool fz = dm.mode != GS_DEPTH_Z;
+        if (variant & 4) rc = fz ? launch(k_preprocess<0, 5, false, true, true>) : launch(k_preprocess<0, 5, false, false, true>);
+        else if (b4) rc = fz ? launch(k_preprocess<2, 5, true, true, true>) : launch(k_preprocess<2, 5, true, false, true>);
+        else if (in.shs) rc = fz ? launch(k_preprocess<2, 5, false, true, true>) : launch(k_preprocess<2, 5, false, false, true>);
+        else rc = fz ? launch(k_preprocess<1, 5, false, true, true>) : launch(k_preprocess<1, 5, false, false, true>);
+    } else if (dm.mode != GS_DEPTH_Z) {   // rec2.w = f(z): the FZ kernels
         if (variant & 4) rc = more_ctas ? launch(k_preprocess<0, 6, false, true>) : launch(k_preprocess<0, 5, false, true>);
         else if (b4) rc = launch(k_preprocess<2, 5, true, true>);
         else if (in.shs) rc = more_ctas ? launch(k_preprocess<2, 6, false, true>) : launch(k_preprocess<2, 5, false, true>);

@@ -188,7 +188,11 @@ __device__ __forceinline__ const float *load_det_acc(const DetAcc &det, size_t o
 // B4: degree 4 (c.deg == 4, M >= 25).  The 48 accumulators of bands 0..3 stay in registers as in the default kernel; the
 // 27 of band 4 live in a shared-memory row per thread next to the staged inputs (stride 27, odd: conflict-free), which
 // keeps the register bound -- and so the 4 resident CTAs per SM -- of the default kernel.
-template <bool HAS_SH, int MINB, int VIEW_Z = 0, bool DET = false, bool B4 = false>
+// AA: the forward ran with GS_FLAG_ANTIALIAS and drew opacity o' = o rho (gs_aa_rho), so the accumulated dL/dopacity is
+// dL/do'.  rho is recomputed from the rebuilt 2-D covariance: dL/do = sum_v rho_v dL/do'_v, and o dL/do' drho/d(a0, b, c0)
+// joins dL/d(a, b, c) ahead of the cov2D -> cov3D and cov2D -> J -> mean chains (DESIGN.md 5.5).  The AA = false kernels
+// are the ones without it, instruction for instruction.
+template <bool HAS_SH, int MINB, int VIEW_Z = 0, bool DET = false, bool B4 = false, bool AA = false>
 __global__ void __launch_bounds__(PB_THREADS, MINB)
 k_preprocess_bwd(const DevCfg c, const DevInputs in, const uint8_t *__restrict__ meta, const float *__restrict__ acc,
                     const GsInGrads g, const DetAcc det, const DepthMode dm) {
@@ -235,8 +239,10 @@ k_preprocess_bwd(const DevCfg c, const DevInputs in, const uint8_t *__restrict__
     float3 mean = make_float3(0, 0, 0);
     float c6[6] = {0, 0, 0, 0, 0, 0};
     float sc[3] = {0, 0, 0}, q[4] = {0, 0, 0, 0};
+    float opac = 0.f;   // AA only: the scene-level opacity o
     if (active) {
         mean = make_float3(in.means3D[sg * 3 + 0], in.means3D[sg * 3 + 1], in.means3D[sg * 3 + 2]);
+        if constexpr (AA) opac = in.opacities[sg];
         if (in.cov3D) {
 #pragma unroll
             for (int k = 0; k < 6; k++) c6[k] = in.cov3D[sg * 6 + k];
@@ -278,7 +284,7 @@ k_preprocess_bwd(const DevCfg c, const DevInputs in, const uint8_t *__restrict__
             gcol[0] = a[0]; gcol[1] = a[1]; gcol[2] = a[2];
             m2d[0] = a[3]; m2d[1] = a[4];
             const float gcx = a[5], gcy = a[6], gcz = a[7];
-            gopac += a[8];
+            if constexpr (!AA) gopac += a[8];
             const float gz = VIEW_Z == 2 ? a[9] * depth_chain(cam, mean, dm, v) : a[9];
             const float s = cam.scale, s2 = s * s;
             const float3 m = make_float3(mean.x * s, mean.y * s, mean.z * s);
@@ -297,10 +303,28 @@ k_preprocess_bwd(const DevCfg c, const DevInputs in, const uint8_t *__restrict__
                 const float denom = aa * cc - bb * bb;
                 const float d2inv = 1.0f / (denom * denom + 0.0000001f);
                 float dL_da = 0.f, dL_db = 0.f, dL_dc = 0.f;
+                // AA: rho as preprocess computed it, and the factor k = o dL/do' h / (2 rho det1^2) of its derivatives
+                float aa_k = 0.f, a0 = 0.f, c0 = 0.f;
+                if constexpr (AA) {
+                    a0 = j.m0[0] * s0[0] + j.m0[1] * s0[1] + j.m0[2] * s0[2];
+                    c0 = j.m1[0] * s1[0] + j.m1[1] * s1[1] + j.m1[2] * s1[2];
+                    const float ratio = gs_aa_ratio(a0, bb, c0, denom);
+                    const float rho = gs_aa_rho(ratio);
+                    gopac += rho * a[8];
+                    // below the clamp rho is a constant
+                    if (ratio > GS_AA_RATIO_MIN) aa_k = opac * a[8] * c.dilation / (2.0f * rho * denom * denom);
+                }
                 if (d2inv != 0.0f) {
                     dL_da = d2inv * (-cc * cc * gcx + 2.0f * bb * cc * gcy + (denom - aa * cc) * gcz);
                     dL_dc = d2inv * (-aa * aa * gcz + 2.0f * aa * bb * gcy + (denom - aa * cc) * gcx);
                     dL_db = d2inv * 2.0f * (bb * cc * gcx - (denom + 2.0f * bb * bb) * gcy + aa * bb * gcz);
+                    if constexpr (AA) {
+                        // ratio = det0 / det1: d/da0 = h (c0 cc + b^2) / det1^2, d/dc0 = h (a0 aa + b^2) / det1^2,
+                        // d/db = -2 b h (aa + c0) / det1^2 (aa = a0 + h, cc = c0 + h)
+                        dL_da += aa_k * (c0 * cc + bb * bb);
+                        dL_dc += aa_k * (a0 * aa + bb * bb);
+                        dL_db -= 2.0f * aa_k * bb * (aa + c0);
+                    }
                     const float *m0 = j.m0, *m1 = j.m1;
                     gcov[0] += s2 * (m0[0] * m0[0] * dL_da + m0[0] * m1[0] * dL_db + m1[0] * m1[0] * dL_dc);
                     gcov[3] += s2 * (m0[1] * m0[1] * dL_da + m0[1] * m1[1] * dL_db + m1[1] * m1[1] * dL_dc);
@@ -768,24 +792,28 @@ k_preprocess_bwd_2phase(const DevCfg c, const DevInputs in, const uint8_t *__res
     }
 }
 
-template <int VIEW_Z, bool DET>
+// AA: the anti-aliased kernels (single pass only: the two-phase kernel has none)
+template <int VIEW_Z, bool DET, bool AA>
 int launch_preprocess_bwd_t(const DevCfg &c, const DevInputs &in, const GsSaved &s, const float *grad_acc,
                             const GsInGrads &g, cudaStream_t st, int variant, const DetAcc &det, const DepthMode &dm) {
     dim3 grid((c.P + PB_THREADS - 1) / PB_THREADS, c.S);
+    if (AA && variant == 1)
+        return gs_set_error(GS_ERR_INVALID, "GS_TUNE_PBWD_2PHASE has no anti-aliased kernel (GS_FLAG_ANTIALIAS)");
     if (in.shs && c.deg > 3) {   // degree 4: the single-pass kernel with band 4 compiled in
         if (variant == 1)
             return gs_set_error(GS_ERR_INVALID, "GS_TUNE_PBWD_2PHASE has no degree-4 kernel (sh_eval_max_degree = 4)");
         const size_t smem = PB_SMEM_HDR + (size_t)PB_THREADS * (c.M * 3 + PB_SH_B4) * 4;
-        auto kern = k_preprocess_bwd<true, PB_MIN_CTAS, VIEW_Z, DET, true>;
+        auto kern = k_preprocess_bwd<true, PB_MIN_CTAS, VIEW_Z, DET, true, AA>;
         GS_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         kern<<<grid, PB_THREADS, smem, st>>>(c, in, s.meta, grad_acc, g, det, dm);
-    } else if (variant != 1) {  // single pass over the views (default)
+    } else if (AA || variant != 1) {  // single pass over the views (default)
         if (in.shs) {
             size_t smem = PB_SMEM_HDR + (size_t)PB_THREADS * c.M * 12;
-            GS_CUDA_OK(cudaFuncSetAttribute(k_preprocess_bwd<true, PB_MIN_CTAS, VIEW_Z, DET>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-            k_preprocess_bwd<true, PB_MIN_CTAS, VIEW_Z, DET><<<grid, PB_THREADS, smem, st>>>(c, in, s.meta, grad_acc, g, det, dm);
+            auto kern = k_preprocess_bwd<true, PB_MIN_CTAS, VIEW_Z, DET, false, AA>;
+            GS_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            kern<<<grid, PB_THREADS, smem, st>>>(c, in, s.meta, grad_acc, g, det, dm);
         } else {
-            k_preprocess_bwd<false, PB_MIN_CTAS, VIEW_Z, DET><<<grid, PB_THREADS, PB_SMEM_HDR, st>>>(c, in, s.meta, grad_acc, g, det, dm);
+            k_preprocess_bwd<false, PB_MIN_CTAS, VIEW_Z, DET, false, AA><<<grid, PB_THREADS, PB_SMEM_HDR, st>>>(c, in, s.meta, grad_acc, g, det, dm);
         }
     } else if (in.shs) {
         size_t smem = PB_SMEM_HDR + (size_t)PB_THREADS * (c.M <= PB_SH_EVAL ? c.M * 3 : PB_SH_EVAL * 3 + 1) * 4;
@@ -811,6 +839,17 @@ __global__ void k_view_z_finalize(int V, int warps, const float *__restrict__ vi
 
 int view_z_warps(const DevCfg &c) { return (c.P + PB_THREADS - 1) / PB_THREADS * (PB_THREADS / 32); }
 
+// the VIEW_Z kernels of one (DET, AA) pair: 2 after a forward whose depth channel carried f(z), else 1 when the view-matrix
+// gradient is wanted, else 0
+template <bool DET, bool AA>
+int launch_preprocess_bwd_vz(const DevCfg &c, const DevInputs &in, const GsSaved &s, const float *grad_acc,
+                             const GsInGrads &g, cudaStream_t st, int variant, const DetAcc &det, const DepthMode &dm) {
+    const bool fz = (s.flags & GS_FLAG_DEPTH) && s.depth_mode != GS_DEPTH_Z;
+    if (fz) return launch_preprocess_bwd_t<2, DET, AA>(c, in, s, grad_acc, g, st, variant, det, dm);
+    return g.dL_dviewmatrix_z ? launch_preprocess_bwd_t<1, DET, AA>(c, in, s, grad_acc, g, st, variant, det, dm)
+                              : launch_preprocess_bwd_t<0, DET, AA>(c, in, s, grad_acc, g, st, variant, det, dm);
+}
+
 }  // namespace
 
 size_t det_view_z_bytes(const DevCfg &c) { return (size_t)c.V * view_z_warps(c) * 4 * sizeof(float); }
@@ -820,17 +859,13 @@ size_t det_view_z_bytes(const DevCfg &c) { return (size_t)c.V * view_z_warps(c) 
 int launch_preprocess_bwd(const DevCfg &c, const DevInputs &in, const GsSaved &s, const float *grad_acc,
                           const GsInGrads &g, cudaStream_t st, int variant, const DetAcc &det, const DepthMode &dm) {
     if (c.P == 0) return GS_OK;
-    // a forward whose depth channel carried f(z): the VIEW_Z = 2 kernels, with or without the view-matrix gradient
-    const bool fz = (s.flags & GS_FLAG_DEPTH) && s.depth_mode != GS_DEPTH_Z;
-    if (!det.acc) {
-        if (fz) return launch_preprocess_bwd_t<2, false>(c, in, s, grad_acc, g, st, variant, det, dm);
-        return g.dL_dviewmatrix_z ? launch_preprocess_bwd_t<1, false>(c, in, s, grad_acc, g, st, variant, det, dm)
-                                  : launch_preprocess_bwd_t<0, false>(c, in, s, grad_acc, g, st, variant, det, dm);
-    }
-    int rc;
-    if (fz) rc = launch_preprocess_bwd_t<2, true>(c, in, s, grad_acc, g, st, variant, det, dm);
-    else if (!g.dL_dviewmatrix_z) return launch_preprocess_bwd_t<0, true>(c, in, s, grad_acc, g, st, variant, det, dm);
-    else rc = launch_preprocess_bwd_t<1, true>(c, in, s, grad_acc, g, st, variant, det, dm);
+    // the forward's anti-aliasing setting, whatever this call's flags say
+    const bool aa = (s.flags & GS_FLAG_ANTIALIAS) != 0;
+    if (!det.acc)
+        return aa ? launch_preprocess_bwd_vz<false, true>(c, in, s, grad_acc, g, st, variant, det, dm)
+                  : launch_preprocess_bwd_vz<false, false>(c, in, s, grad_acc, g, st, variant, det, dm);
+    const int rc = aa ? launch_preprocess_bwd_vz<true, true>(c, in, s, grad_acc, g, st, variant, det, dm)
+                      : launch_preprocess_bwd_vz<true, false>(c, in, s, grad_acc, g, st, variant, det, dm);
     if (rc != GS_OK || !g.dL_dviewmatrix_z) return rc;
     k_view_z_finalize<<<(c.V * 4 + 127) / 128, 128, 0, st>>>(c.V, view_z_warps(c), det.view_z, g.dL_dviewmatrix_z);
     GS_CUDA_OK(cudaGetLastError());

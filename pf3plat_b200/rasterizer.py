@@ -172,6 +172,10 @@ class BatchSettings(NamedTuple):
     # view-scaled scene), "disparity", "relative_disparity" or "log" (f(z) of render_depth_cuda at the unscaled z)
     depth_mode: str = "depth"
     depth_near_far: Optional[torch.Tensor] = None  # (V,2) unscaled near, far: needed by "relative_disparity" and "log"
+    # anti-aliasing (GS_FLAG_ANTIALIAS): the screen-space filter with opacity compensation -- each splat drawn at opacity
+    # o * rho, rho = sqrt(det Sigma2 / det(Sigma2 + dilation I)) per (view, Gaussian); None = the process-wide setting
+    # (set_antialiasing, default off)
+    antialiasing: Optional[bool] = None
     # also return the accumulated opacity alpha = 1 - T_final (V,H,W) of the colour pass (GsAlpha); its gradient reaches
     # the geometry and the opacities, never SH, colours or cameras
     with_alpha: bool = False
@@ -205,10 +209,40 @@ def _check_degree(degree) -> int:
 
 
 def _resolve_degree(bs: BatchSettings) -> BatchSettings:
-    """bs with sh_eval_max_degree made explicit (the process-wide setting in place of None)."""
+    """bs with sh_eval_max_degree and antialiasing made explicit (the process-wide settings in place of None)."""
     if bs.sh_eval_max_degree is None:
-        return bs._replace(sh_eval_max_degree=_sh_eval_max_degree)
+        bs = bs._replace(sh_eval_max_degree=_sh_eval_max_degree)
+    if bs.antialiasing is None:
+        bs = bs._replace(antialiasing=_antialiasing)
     return bs
+
+
+# ---------------------------------------------------------------------------------------------------------
+# anti-aliasing, for callers that cannot pass BatchSettings (the drop-in GaussianRasterizer, an unmodified render_cuda)
+# ---------------------------------------------------------------------------------------------------------
+_antialiasing = False
+
+
+def set_antialiasing(enabled: bool) -> None:
+    """Process-wide anti-aliasing setting used when BatchSettings.antialiasing (or the `antialiasing` argument of the
+    drop-in, render_views, decoder_forward) is None: False (the default, upstream's default behaviour) or True (the
+    screen-space filter with opacity compensation, upstream's `antialiasing=True`).  A forward's backward differentiates
+    what that forward rendered, whatever the setting is by then."""
+    global _antialiasing
+    enabled = bool(enabled)
+    if enabled:
+        _check_antialias_supported()
+    _antialiasing = enabled
+
+
+def get_antialiasing() -> bool:
+    return _antialiasing
+
+
+def _check_antialias_supported() -> None:
+    # a library that predates the flag ignores the bit instead of refusing it: ask it what it honours
+    if not _capi.lib().gs_supported_flags() & _capi.GS_FLAG_ANTIALIAS:
+        raise RuntimeError(f"{_capi.LIB_PATH} does not support anti-aliasing (GS_FLAG_ANTIALIAS): rebuild it")
 
 
 def _make_config(bs: BatchSettings, S: int, P: int, M: int, keep: list) -> GsConfig:
@@ -219,6 +253,9 @@ def _make_config(bs: BatchSettings, S: int, P: int, M: int, keep: list) -> GsCon
     cfg.sh_degree = int(bs.sh_degree)
     cfg.image_height, cfg.image_width = int(bs.image_height), int(bs.image_width)
     cfg.flags = (_capi.GS_FLAG_DEPTH if bs.with_depth else 0) | (_capi.GS_FLAG_PREFILTERED if bs.prefiltered else 0)
+    if _antialiasing if bs.antialiasing is None else bs.antialiasing:
+        _check_antialias_supported()
+        cfg.flags |= _capi.GS_FLAG_ANTIALIAS
     cfg.tanfovx, cfg.tanfovy = float(bs.tanfovx), float(bs.tanfovy)
     cfg.scale_modifier = float(bs.scale_modifier)
     cfg.tuning = int(bs.tuning)
@@ -427,13 +464,17 @@ class GaussianRasterizer(nn.Module):
             return present.bool()
 
     def forward(self, means3D, means2D, opacities, shs=None, colors_precomp=None, scales=None, rotations=None,
-                cov3D_precomp=None, return_depth: bool = False, return_alpha: bool = False):
+                cov3D_precomp=None, return_depth: bool = False, return_alpha: bool = False,
+                antialiasing: Optional[bool] = None):
         """Returns (color (3,H,W), radii (P,)) like the reference op; `return_depth=True` (opt-in, not used by
         PF3plat) appends the composited camera-space depth (H,W), `return_alpha=True` then the accumulated opacity
-        1 - T_final (H,W)."""
+        1 - T_final (H,W).  `antialiasing`: the screen-space filter with opacity compensation (upstream's
+        GaussianRasterizationSettings.antialiasing, which this 12-field settings tuple does not carry); None = the
+        process-wide setting (set_antialiasing)."""
         _check_exclusive(shs, colors_precomp, scales, rotations, cov3D_precomp)
         u = lambda t: None if t is None else t.unsqueeze(0)
-        bs = self._batch_settings(means3D.device, with_depth=return_depth)._replace(with_alpha=bool(return_alpha))
+        bs = self._batch_settings(means3D.device, with_depth=return_depth)._replace(
+            with_alpha=bool(return_alpha), antialiasing=None if antialiasing is None else bool(antialiasing))
         out = _RasterizeBatch.apply(u(means3D), u(means2D), u(shs), u(colors_precomp), u(opacities), u(scales),
                                     u(rotations), u(cov3D_precomp), bs.viewmatrix, bs)
         return tuple(o[0] for o in out)

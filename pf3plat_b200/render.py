@@ -33,7 +33,8 @@ def _cov6(cov: torch.Tensor) -> torch.Tensor:
 def render_views(extrinsics, intrinsics, near, far, image_shape, background_color, gaussian_means,
                  gaussian_covariances, gaussian_sh_coefficients, gaussian_opacities, scale_invariant: bool = True,
                  use_sh: bool = True, with_depth: bool = False, sh_layout: str = "g_xyz_n",
-                 sh_eval_max_degree: Optional[int] = None, depth_mode: str = "depth", with_alpha: bool = False):
+                 sh_eval_max_degree: Optional[int] = None, depth_mode: str = "depth", with_alpha: bool = False,
+                 antialiasing: Optional[bool] = None):
     """extrinsics (B,4,4) c2w, intrinsics (B,3,3), near/far (B,), background (B,3); Gaussians are per SCENE and NOT
     repeated per view: means (S,G,3), covariances (S,G,3,3) or (S,G,6), sh (S,G,3,d_sh) [or (S,G,d_sh,3) with
     sh_layout="g_n_xyz"], opacities (S,G); B % S == 0 and view b shows scene b // (B//S).
@@ -42,7 +43,9 @@ def render_views(extrinsics, intrinsics, near, far, image_shape, background_colo
     Returns color (B,3,h,w) and, if with_depth, depth (B,h,w) = sum_i alpha_i T_i f(z_i): f(z) = z of the (rescaled)
     scene for depth_mode "depth"; for "disparity", "relative_disparity" and "log" the fake colour of render_depth_cuda
     (cuda_splatting.py:245-251) at the UNSCALED camera-space depth z, with the unscaled near and far.
-    with_alpha: also return the accumulated opacity alpha (B,h,w) = 1 - T_final, last: (color[, depth], alpha)."""
+    with_alpha: also return the accumulated opacity alpha (B,h,w) = 1 - T_final, last: (color[, depth], alpha).
+    antialiasing: the screen-space filter with opacity compensation (BatchSettings.antialiasing); None = the
+    process-wide setting (rasterizer.set_antialiasing, default off)."""
     assert use_sh or gaussian_sh_coefficients.shape[-1 if sh_layout == "g_xyz_n" else -2] == 1
     h, w = image_shape
     vb = make_view_batch(extrinsics, intrinsics, near, far, scale_invariant)
@@ -60,7 +63,7 @@ def render_views(extrinsics, intrinsics, near, far, image_shape, background_colo
                        view_scale=vb.scale if scale_invariant else None, with_depth=with_depth,
                        sh_eval_max_degree=sh_eval_max_degree, depth_mode=depth_mode,
                        depth_near_far=torch.stack([near, far], -1) if with_depth and depth_mode != "depth" else None,
-                       with_alpha=with_alpha)
+                       with_alpha=with_alpha, antialiasing=antialiasing)
     B = extrinsics.shape[0]
     S = gaussian_means.shape[0]
     if use_sh:
@@ -86,7 +89,7 @@ def render_cuda(extrinsics, intrinsics, near, far, image_shape, background_color
 
 def decoder_forward(means, covariances, harmonics, opacities, extrinsics, intrinsics, near, far, image_shape,
                     background_color, depth_mode: Optional[str] = None, sh_eval_max_degree: Optional[int] = None,
-                    return_alpha: bool = False):
+                    return_alpha: bool = False, antialiasing: Optional[bool] = None):
     """`DecoderSplattingCUDA.forward` (decoder_splatting_cuda.py:35-67) without the v-fold repeat: Gaussians
     (b,g,...), cameras (b,v,...).  Returns (color (b,v,3,h,w), depth (b,v,h,w) or None).  Every depth_mode of the
     reference ("depth", "disparity", "relative_disparity", "log") is composited in the same pass as the colour.
@@ -100,13 +103,15 @@ def decoder_forward(means, covariances, harmonics, opacities, extrinsics, intrin
     read the depth leaves the extrinsics without a gradient, as the reference does.  So every mode is one render whether
     or not the extrinsics require grad.  sh_eval_max_degree: as render_views.
     return_alpha: also return the accumulated opacity (b,v,h,w) = 1 - T_final of the same pass, as (color, depth, alpha)
-    (depth None without a depth_mode).  It trains the Gaussians' geometry and opacities, never the extrinsics."""
+    (depth None without a depth_mode).  It trains the Gaussians' geometry and opacities, never the extrinsics.
+    antialiasing: as render_views; the opacity compensation gives the extrinsics no gradient either."""
     b, v = extrinsics.shape[:2]
     flat = lambda t: t.reshape(b * v, *t.shape[2:])
     bg = background_color.reshape(1, 3).expand(b * v, 3)
     out = render_views(flat(extrinsics), flat(intrinsics), flat(near), flat(far), image_shape, bg, means,
                        covariances, harmonics, opacities, with_depth=depth_mode is not None,
-                       sh_eval_max_degree=sh_eval_max_degree, depth_mode=depth_mode or "depth", with_alpha=return_alpha)
+                       sh_eval_max_degree=sh_eval_max_degree, depth_mode=depth_mode or "depth", with_alpha=return_alpha,
+                       antialiasing=antialiasing)
     alpha = None
     if return_alpha:
         *out, alpha = out

@@ -406,20 +406,30 @@ GS_API int gs_photometric_backward(const GsLossConfig *cfg, const float *predict
  * there for gs_lpips_backward, which must get the same config and workspace.  out [batch] (the package's (N,1,1,1)).
  * dL_dout [batch] is a device array; dL_din0 / dL_din1 are written contiguous [batch, 3, height, width], NULL = not
  * wanted (each needs its bit in grads).  Deterministic (no atomics), no host synchronisation.
+ * precision GS_LPIPS_BF16 (opt-in) runs BF16 activations and inter-layer gradients with BF16 wgmma convolutions (fp32
+ * accumulation), as torch.autocast(dtype=torch.bfloat16) would; inputs, out and dL_din stay fp32.  It needs
+ * gs_lpips_weights_pack_bf16 on the handle first (GS_ERR_INVALID otherwise), which adds BF16 copies of the conv weights
+ * (about 59 MB) from the same fp32 conv_weight[13] (only [1..12] are read); a handle packed already is left as it is.
  */
 typedef struct GsLpipsWeights GsLpipsWeights;
+
+enum { GS_LPIPS_TF32 = 0, GS_LPIPS_BF16 = 1 };
 
 typedef struct GsLpipsConfig {
     int32_t batch, height, width;
     int32_t normalize;              /* 0 or 1: inputs are mapped x -> 2x - 1 first (the package's normalize=True) */
     int64_t in0_stride, in1_stride; /* floats between consecutive images (ignored when batch == 1) */
     int32_t grads;                  /* bit 0: dL/din0 will be wanted, bit 1: dL/din1; 0 = forward only */
-    int32_t reserved_;
+    union {
+        int32_t precision; /* GS_LPIPS_TF32 (0, the default) or GS_LPIPS_BF16; the workspace size depends on it */
+        int32_t reserved_; /* the field's name before it held the precision */
+    };
 } GsLpipsConfig;
 
 GS_API int gs_lpips_weights_create(const float *const *conv_weight /* [13] */, const float *const *conv_bias /* [13] */,
                                    const float *const *lin /* [5] */, const float *shift, const float *scale, void *stream,
                                    GsLpipsWeights **out);
+GS_API int gs_lpips_weights_pack_bf16(GsLpipsWeights *weights, const float *const *conv_weight /* [13] */, void *stream);
 GS_API void gs_lpips_weights_destroy(GsLpipsWeights *weights);
 GS_API int64_t gs_lpips_workspace_bytes(const GsLpipsConfig *cfg); /* -1 for an invalid config */
 GS_API int gs_lpips_forward(const GsLpipsWeights *weights, const GsLpipsConfig *cfg, const float *in0, const float *in1,

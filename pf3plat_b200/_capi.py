@@ -121,9 +121,16 @@ class GsLossConfig(Structure):
                 ("pred_stride", c_int64), ("gt_stride", c_int64), ("with_mse", c_int32), ("reserved_", c_int32)]
 
 
+GS_LPIPS_TF32, GS_LPIPS_BF16 = 0, 1
+LPIPS_PRECISIONS = {"tf32": GS_LPIPS_TF32, "bf16": GS_LPIPS_BF16}
+
+
 class GsLpipsConfig(Structure):
     _fields_ = [("batch", c_int32), ("height", c_int32), ("width", c_int32), ("normalize", c_int32),
-                ("in0_stride", c_int64), ("in1_stride", c_int64), ("grads", c_int32), ("reserved_", c_int32)]
+                ("in0_stride", c_int64), ("in1_stride", c_int64), ("grads", c_int32), ("precision", c_int32)]
+
+
+GsLpipsConfig.reserved_ = GsLpipsConfig.precision  # the header's other name for the field (a union member)
 
 
 SYMBOLS = {
@@ -163,6 +170,7 @@ SYMBOLS = {
                                         c_void_p, c_void_p]),
     "gs_lpips_weights_create": (c_int, [POINTER(c_void_p), POINTER(c_void_p), POINTER(c_void_p), c_void_p, c_void_p,
                                         c_void_p, POINTER(c_void_p)]),
+    "gs_lpips_weights_pack_bf16": (c_int, [c_void_p, POINTER(c_void_p), c_void_p]),
     "gs_lpips_weights_destroy": (None, [c_void_p]),
     "gs_lpips_workspace_bytes": (c_int64, [POINTER(GsLpipsConfig)]),
     "gs_lpips_forward": (c_int, [c_void_p, POINTER(GsLpipsConfig), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),

@@ -11,6 +11,12 @@ the installed `lpips` package, as the reference does.  The module holds them und
 `load_state_dict` and convert_to_buffer keep working; they are packed into the kernels' layouts lazily, once per device,
 and packed again whenever a weight tensor is replaced or modified in place.  Inputs must be float32 CUDA tensors of at
 least 16 x 16 pixels; there is no CPU fallback.
+
+Precision: `precision="tf32"` (the default) is the path above.  `precision="bf16"` is an opt-in for the training loss:
+BF16 activations and inter-layer gradients, BF16 wgmma convolutions with fp32 accumulation -- what torch.autocast with
+bfloat16 gives the `lpips` package -- at about half the convolution time; inputs, outputs and input gradients stay
+float32.  `precision=None` follows the process-wide setting (`set_precision`, default "tf32"), so a caller that builds
+`LPIPS(net="vgg")` itself can opt in without changing that call.  torch.autocast is not consulted.
 """
 from __future__ import annotations
 
@@ -30,6 +36,26 @@ _SLICE_ENDS = (4, 9, 16, 23, 30)
 _TAP_CHANNELS = (64, 128, 256, 512, 512)
 _SHIFT = (-.030, -.088, -.188)
 _SCALE = (.458, .448, .450)
+
+
+_precision = "tf32"
+
+
+def _check_precision(precision) -> str:
+    if precision not in _capi.LPIPS_PRECISIONS:
+        raise ValueError(f"LPIPS precision must be one of {sorted(_capi.LPIPS_PRECISIONS)}, got {precision!r}")
+    return precision
+
+
+def set_precision(precision: str) -> None:
+    """Process-wide precision of LPIPS modules built with precision=None: "tf32" (the default) or "bf16".  A forward's
+    backward runs in the precision of that forward, whatever the setting is by then."""
+    global _precision
+    _precision = _check_precision(precision)
+
+
+def get_precision() -> str:
+    return _precision
 
 
 def _slice_of(idx: int) -> int:
@@ -92,9 +118,10 @@ def canonical_state_dict(sd: dict) -> dict:
 
 
 class _Pack:
-    """Packed weights on one device (gs_lpips_weights_create); freed with the object."""
+    """Packed weights on one device (gs_lpips_weights_create, plus gs_lpips_weights_pack_bf16 for "bf16"); freed with
+    the object."""
 
-    def __init__(self, tensors, device):
+    def __init__(self, tensors, device, precision):
         L = _capi.lib()
         # float32 copies on the device; packing is stream-ordered, so they may be freed once it is enqueued
         src = [t.detach().to(device, torch.float32).contiguous() for t in tensors]
@@ -106,7 +133,9 @@ class _Pack:
         with torch.cuda.device(device):
             _capi.check(L.gs_lpips_weights_create(cw, cb, lin, ptrs[31], ptrs[32],
                                                   torch.cuda.current_stream(device).cuda_stream, ctypes.byref(handle)))
-        self.handle = handle.value
+            self.handle = handle.value
+            if precision == "bf16":
+                _capi.check(L.gs_lpips_weights_pack_bf16(self.handle, cw, torch.cuda.current_stream(device).cuda_stream))
 
     def __del__(self):
         if getattr(self, "handle", None):
@@ -116,12 +145,12 @@ class _Pack:
 
 class _LpipsFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, in0, in1, pack, normalize, grads):
+    def forward(ctx, in0, in1, pack, normalize, grads, precision):
         a, n, chw, sa = _layout(in0)
         b, _, _, sb = _layout(in1)
         _, h, w = chw
         cfg = _capi.GsLpipsConfig(batch=n, height=h, width=w, normalize=int(bool(normalize)), in0_stride=sa, in1_stride=sb,
-                                  grads=grads)
+                                  grads=grads, precision=_capi.LPIPS_PRECISIONS[precision])
         dev = in0.device
         L = _capi.lib()
         out = torch.empty((n,), dtype=torch.float32, device=dev)
@@ -141,7 +170,7 @@ class _LpipsFn(torch.autograd.Function):
     def backward(ctx, dout):
         need0, need1 = ctx.needs_input_grad[:2]
         if dout is None or not (need0 or need1):
-            return None, None, None, None, None
+            return None, None, None, None, None, None
         cfg, dev = ctx.cfg, dout.device
         n, h, w = cfg.batch, cfg.height, cfg.width
         g0 = torch.empty((n, 3, h, w), dtype=torch.float32, device=dev) if need0 else None
@@ -153,17 +182,19 @@ class _LpipsFn(torch.autograd.Function):
                 _capi.check(_capi.lib().gs_lpips_backward(ctx.pack.handle, ctypes.byref(cfg), d.data_ptr(), ctx.ws.data_ptr(),
                                                           ptr(g0), ptr(g1), torch.cuda.current_stream(dev).cuda_stream))
         s0, s1 = ctx.shapes
-        return (g0.reshape(s0) if g0 is not None else None), (g1.reshape(s1) if g1 is not None else None), None, None, None
+        return (g0.reshape(s0) if g0 is not None else None), (g1.reshape(s1) if g1 is not None else None), None, None, None, None
 
 
 class LPIPS(nn.Module):
     """LPIPS(net="vgg") of the `lpips` package on the device.  forward(in0, in1, retPerLayer=False, normalize=False)
-    -> (N, 1, 1, 1) for (N, 3, H, W) inputs ((B, V, 1, 1, 1) for (B, V, 3, H, W))."""
+    -> (N, 1, 1, 1) for (N, 3, H, W) inputs ((B, V, 1, 1, 1) for (B, V, 3, H, W)).  precision: "tf32", "bf16" or None
+    (the process-wide setting of set_precision at each forward)."""
 
-    def __init__(self, net: str = "vgg", weights=None, **unused_package_options):
+    def __init__(self, net: str = "vgg", weights=None, precision=None, **unused_package_options):
         super().__init__()
         if net != "vgg":
             raise NotImplementedError(f"only net='vgg' is implemented, got {net!r}")
+        self.precision = None if precision is None else _check_precision(precision)
         self.scaling_layer = _Scaling()
         self.net = nn.Module()
         for k in range(1, 6):
@@ -186,16 +217,16 @@ class LPIPS(nn.Module):
         keys = [k for pair in CONV_KEYS for k in pair] + list(LIN_KEYS) + ["scaling_layer.shift", "scaling_layer.scale"]
         return [get(k) for k in keys]
 
-    def _pack(self, device) -> _Pack:
-        """The packed weights for `device`, packed again if any weight tensor was replaced or changed in place (the
-        cache holds the tensors it packed, so identity and version counter decide)."""
+    def _pack(self, device, precision="tf32") -> _Pack:
+        """The packed weights for (`device`, `precision`), packed again if any weight tensor was replaced or changed in
+        place (the cache holds the tensors it packed, so identity and version counter decide)."""
         tensors = self._tensors()
         sig = [(t, t._version) for t in tensors]
-        hit = self._packs.get(device)
+        hit = self._packs.get((device, precision))
         if hit is not None and len(hit[0]) == len(sig) and all(a is b and va == vb for (a, va), (b, vb) in zip(hit[0], sig)):
             return hit[1]
-        pack = _Pack(tensors, device)
-        self._packs[device] = (sig, pack)
+        pack = _Pack(tensors, device, precision)
+        self._packs[(device, precision)] = (sig, pack)
         return pack
 
     def forward(self, in0: torch.Tensor, in1: torch.Tensor, retPerLayer: bool = False, normalize: bool = False):
@@ -212,5 +243,6 @@ class LPIPS(nn.Module):
             raise ValueError(f"LPIPS needs 3-channel images of at least 16 x 16 pixels, got {tuple(in0.shape)}")
         # which input gradients the backward may be asked for decides what the forward keeps
         grads = (int(in0.requires_grad) | 2 * int(in1.requires_grad)) if torch.is_grad_enabled() else 0
-        out = _LpipsFn.apply(in0, in1, self._pack(in0.device), normalize, grads)
+        precision = _precision if self.precision is None else self.precision
+        out = _LpipsFn.apply(in0, in1, self._pack(in0.device, precision), normalize, grads, precision)
         return out.reshape(tuple(in0.shape[:-3]) + (1, 1, 1))

@@ -38,8 +38,9 @@ def compute_psnr(ground_truth: torch.Tensor, predicted: torch.Tensor) -> torch.T
 
 @functools.cache
 def get_lpips(device: torch.device) -> LPIPS:
-    """One LPIPS-VGG module per device (metrics.py:22-24)."""
-    return LPIPS(net="vgg").to(device)
+    """One LPIPS-VGG module per device (metrics.py:22-24), in TF32 whatever lpips.set_precision says: a reported metric
+    does not depend on a training-speed setting."""
+    return LPIPS(net="vgg", precision="tf32").to(device)
 
 
 @torch.no_grad()

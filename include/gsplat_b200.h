@@ -249,6 +249,28 @@ GS_API int gs_forward_ex(GsContext *ctx, const GsConfig *cfg, const GsInputs *in
 GS_API int gs_backward_ex(GsContext *ctx, const GsConfig *cfg, const GsInputs *in, const GsSaved *saved,
                           const GsOutGrads *gout, const GsAlpha *alpha, const GsInGrads *gin, void *stream);
 
+/* Camera gradient, opt-in (gs_backward_cam): dL/d of the three camera inputs of GsConfig, per view and in their own
+ * layouts -- the exact partial derivatives of what the kernels compute, everything else held fixed.  They take in every
+ * output of the forward: colour (from SH or colors_precomp), the depth channel in every depth_mode (through f'(z);
+ * GS_DEPTH_LOG's clamp gives zero), the accumulated opacity and the anti-aliasing factor.  A guard-band-clamped t.x / t.y
+ * has no gradient, an invisible or culled (view, Gaussian) pair contributes nothing, and the 0.99 alpha clamp passes the
+ * gradient straight through, as for the means.  The values are in the view-scaled scene (GsConfig.view_scale), so they
+ * are gradients of the matrices as passed; tanfov, near, far, bg and the intrinsics get none.  Each pointer is device
+ * memory or NULL (not wanted); the arrays are written, not accumulated.  Deterministic: per-warp partials summed in a
+ * fixed order, in both modes. */
+typedef struct GsCameraGrads {
+    float *dL_dviewmatrix;  /* device [V,16]: the flat transposed world-to-camera matrix (GsConfig.viewmatrix) */
+    float *dL_dprojmatrix;  /* device [V,16]: the flat transposed full projection (GsConfig.projmatrix) */
+    float *dL_dcampos;      /* device [V,3] (GsConfig.campos) */
+} GsCameraGrads;
+
+/* gs_backward_ex that also writes the camera gradient (cam, not NULL).  alpha may be NULL (no incoming dL/dalpha).  It
+ * contains the depth channel's z column, so gin->dL_dviewmatrix_z must be NULL (else GS_ERR_INVALID).  GS_TUNE_PBWD_2PHASE
+ * has no camera-gradient kernel: GS_ERR_INVALID. */
+GS_API int gs_backward_cam(GsContext *ctx, const GsConfig *cfg, const GsInputs *in, const GsSaved *saved,
+                           const GsOutGrads *gout, const GsAlpha *alpha, const GsInGrads *gin, const GsCameraGrads *cam,
+                           void *stream);
+
 GS_API void gs_saved_free(GsContext *ctx, GsSaved *saved, void *stream);
 
 /* GaussianRasterizer.markVisible (unused by PF3plat; kept for surface completeness): present[V,P] = in frustum. */

@@ -82,6 +82,11 @@ class GsAlpha(Structure):
     _fields_ = [("alpha", c_void_p), ("dL_dalpha", c_void_p)]
 
 
+class GsCameraGrads(Structure):
+    """The camera gradient gs_backward_cam writes: dL/dviewmatrix [V,16], dL/dprojmatrix [V,16], dL/dcampos [V,3]."""
+    _fields_ = [("dL_dviewmatrix", c_void_p), ("dL_dprojmatrix", c_void_p), ("dL_dcampos", c_void_p)]
+
+
 class GsStats(Structure):
     _fields_ = [("num_rendered", c_int64), ("num_visible", c_int64), ("saved_bytes", c_int64),
                 ("scratch_bytes", c_int64), ("kernel_launches", c_int32), ("max_tile_list", c_int32),
@@ -151,6 +156,8 @@ SYMBOLS = {
                               POINTER(c_void_p), c_void_p]),
     "gs_backward_ex": (c_int, [c_void_p, POINTER(GsConfig), POINTER(GsInputs), c_void_p, POINTER(GsOutGrads),
                                POINTER(GsAlpha), POINTER(GsInGrads), c_void_p]),
+    "gs_backward_cam": (c_int, [c_void_p, POINTER(GsConfig), POINTER(GsInputs), c_void_p, POINTER(GsOutGrads),
+                                POINTER(GsAlpha), POINTER(GsInGrads), POINTER(GsCameraGrads), c_void_p]),
     "gs_render_host_ex": (c_int, [c_void_p, POINTER(GsConfig), POINTER(GsInputs), POINTER(GsOutputs), POINTER(GsAlpha),
                                   c_void_p]),
     "gs_set_profiling": (c_int, [c_void_p, c_int]),

@@ -60,15 +60,21 @@ class ViewBatch:
     scale: torch.Tensor        # (V,) the 1/near rescale applied to means/covariances (1 if not scale-invariant)
 
 
-def make_view_batch(extrinsics, intrinsics, near, far, scale_invariant: bool = True) -> ViewBatch:
+def make_view_batch(extrinsics, intrinsics, near, far, scale_invariant: bool = True,
+                    camera_gradients=None) -> ViewBatch:
     """cuda_splatting.py:64-87 for all views at once (no per-view `.item()` host syncs).
 
     On CUDA tensors whose extrinsics require grad, `viewmatrix` is differentiable w.r.t. them: its values are the
     kernel's, its gradient that of the view matrix built in torch.  This is what lets the fused depth channel carry
     render_depth_cuda's camera gradient (cuda_splatting.py:239-242).  `projmatrix`, `campos` and `tanfov` stay
-    detached, and `near` / `far` get no gradient."""
+    detached, and `near` / `far` get no gradient.
+
+    camera_gradients (None = rasterizer.get_camera_gradients()): on, the three camera inputs follow render_cuda's own
+    torch glue instead -- the translation of the extrinsics rescaled by 1/near, then inverted; projmatrix = view @ P with
+    P detached; campos = the rescaled translation -- so that the full camera gradient reaches the extrinsics in all 16
+    entries as that glue would carry it."""
     if extrinsics.is_cuda:
-        return _make_view_batch_cuda(extrinsics, intrinsics, near, far, scale_invariant)
+        return _make_view_batch_cuda(extrinsics, intrinsics, near, far, scale_invariant, camera_gradients)
     if scale_invariant:
         scale = 1.0 / near
         extrinsics = extrinsics.clone()
@@ -87,7 +93,7 @@ def make_view_batch(extrinsics, intrinsics, near, far, scale_invariant: bool = T
                      scale.contiguous())
 
 
-def _make_view_batch_cuda(extrinsics, intrinsics, near, far, scale_invariant: bool) -> ViewBatch:
+def _make_view_batch_cuda(extrinsics, intrinsics, near, far, scale_invariant: bool, camera_gradients=None) -> ViewBatch:
     import ctypes
 
     from . import _capi
@@ -105,7 +111,26 @@ def _make_view_batch_cuda(extrinsics, intrinsics, near, far, scale_invariant: bo
         _capi.check(_capi.lib().gs_view_batch(B, int(bool(scale_invariant)), p(ext), p(intr), p(nr), p(fr), p(view), p(proj),
                                               p(campos), p(tanfov), p(scale),
                                               ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)))
-    if extrinsics.requires_grad and torch.is_grad_enabled():
+    if camera_gradients is None:
+        from .rasterizer import get_camera_gradients
+        camera_gradients = get_camera_gradients()
+    if camera_gradients and extrinsics.requires_grad and torch.is_grad_enabled():
+        # The kernel's values (plus exact zeros) with the gradients of render_cuda's glue (cuda_splatting.py:64-86)
+        e = extrinsics.clone()
+        inv_near = (1.0 / near.detach().to(dev, e.dtype))
+        if scale_invariant:
+            e[..., :3, 3] = e[..., :3, 3] * inv_near[:, None]
+        vt = torch.linalg.inv(e).transpose(-1, -2)
+        with torch.no_grad():
+            nr_s, fr_s = (nr * scale, fr * scale) if scale_invariant else (nr, fr)
+            fov_x, fov_y = get_fov(intr).unbind(-1)
+            pt = get_projection_matrix(nr_s, fr_s, fov_x, fov_y).transpose(-1, -2).to(vt.dtype)
+        full = vt @ pt
+        cp = e[:, :3, 3]
+        view = view + (vt - vt.detach()).to(view.dtype)
+        proj = proj + (full - full.detach()).to(proj.dtype)
+        campos = campos + (cp - cp.detach()).to(campos.dtype)
+    elif extrinsics.requires_grad and torch.is_grad_enabled():
         # The kernel's values (plus exact zeros) with the gradient of a torch expression of the view matrix.  The
         # expression rescales the translation of extrinsics^-1 rather than that of the extrinsics
         # (cuda_splatting.py:64-86).  Both are equal while the bottom row is (0, 0, 0, 1), but only this one differentiates

@@ -652,7 +652,7 @@ extern "C" int gs_forward_ex(GsContext *ctx, const GsConfig *cfg, const GsInputs
 
 namespace {
 int backward(GsContext *ctx, const GsConfig *cfg, const GsInputs *in, const GsSaved *saved, const GsOutGrads *gout,
-             const float *dL_dalpha, const GsInGrads *gin, void *stream) {
+             const float *dL_dalpha, const GsInGrads *gin, void *stream, const GsCameraGrads *cam = nullptr) {
     if (!ctx || !saved || !gout || !gin) return gs_set_error(GS_ERR_INVALID, "null argument");
     int rc = validate(cfg, in);
     if (rc != GS_OK) return rc;
@@ -664,6 +664,11 @@ int backward(GsContext *ctx, const GsConfig *cfg, const GsInputs *in, const GsSa
         return gs_set_error(GS_ERR_INVALID, "saved state does not match the configuration");
     c.flags = saved->flags;   // (GS_FLAG_ANTIALIAS included: the backward differentiates what its forward drew)
     if ((rc = validate_antialias(c.flags, cfg->tuning, AA_BWD_KNOBS)) != GS_OK) return rc;
+    if (cam && gin->dL_dviewmatrix_z)
+        return gs_set_error(GS_ERR_INVALID, "dL_dviewmatrix_z and GsCameraGrads in one call: the camera gradient already "
+                                            "contains the depth channel's z column");
+    if (cam && (cfg->tuning & GS_TUNE_PBWD_2PHASE))
+        return gs_set_error(GS_ERR_INVALID, "GS_TUNE_PBWD_2PHASE has no camera-gradient kernel (GsCameraGrads)");
     if (gin->dL_dviewmatrix_z && !(c.flags & GS_FLAG_DEPTH))
         return gs_set_error(GS_ERR_INVALID, "dL_dviewmatrix_z needs a forward with GS_FLAG_DEPTH");
     // the forward's depth mode, with this call's near / far
@@ -688,16 +693,25 @@ int backward(GsContext *ctx, const GsConfig *cfg, const GsInputs *in, const GsSa
         if (!gout->dL_ddepth) g.dL_dviewmatrix_z = nullptr;
     }
     const size_t n = (size_t)c.V * c.P;
-    if (n == 0) return GS_OK;
+    if (n == 0) {
+        // no pair contributes: the camera gradient is zero
+        if (cam && cam->dL_dviewmatrix) GS_CUDA_OK(cudaMemsetAsync(cam->dL_dviewmatrix, 0, (size_t)c.V * 16 * 4, st));
+        if (cam && cam->dL_dprojmatrix) GS_CUDA_OK(cudaMemsetAsync(cam->dL_dprojmatrix, 0, (size_t)c.V * 16 * 4, st));
+        if (cam && cam->dL_dcampos) GS_CUDA_OK(cudaMemsetAsync(cam->dL_dcampos, 0, (size_t)c.V * 3 * 4, st));
+        return GS_OK;
+    }
 
     // Accumulators: n x GS_ACC_STRIDE floats; deterministic mode: n x GS_ACC_STRIDE x 3 int64 limbs + n poison masks
-    // (zeroed together), then the per-warp partials of the view-matrix gradient
+    // (zeroed together), then the per-warp partials of the view-matrix gradient; with the camera gradient, its per-warp
+    // partials, in both modes
     const size_t acc_bytes = det ? n * (GS_ACC_STRIDE * GS_DET_LIMBS * 8 + 4) : n * GS_ACC_STRIDE * 4;
     const size_t vz_off = align256(acc_bytes);
-    rc = ctx->per_gaussian.reserve(det ? vz_off + det_view_z_bytes(c) : acc_bytes, 1.0, ctx->pool, st);
+    const size_t vz_bytes = cam ? camera_grad_scratch_bytes(c) : det ? det_view_z_bytes(c) : 0;
+    rc = ctx->per_gaussian.reserve(vz_bytes ? vz_off + vz_bytes : acc_bytes, 1.0, ctx->pool, st);
     if (rc != GS_OK) return rc;
     float *acc = static_cast<float *>(ctx->per_gaussian.p);
     DetAcc da{};
+    if (cam) da.view_z = reinterpret_cast<float *>(static_cast<unsigned char *>(ctx->per_gaussian.p) + vz_off);
     if (det) {
         unsigned char *base = static_cast<unsigned char *>(ctx->per_gaussian.p);
         da.acc = reinterpret_cast<unsigned long long *>(base);
@@ -714,11 +728,12 @@ int backward(GsContext *ctx, const GsConfig *cfg, const GsInputs *in, const GsSa
     }
     {
         StageTimer t(ctx, GS_STAGE_PREPROCESS_BWD, st);
-        rc = launch_preprocess_bwd(c, di, *saved, acc, g, st, (cfg->tuning & GS_TUNE_PBWD_2PHASE) ? 1 : 0, da, dm);
+        rc = launch_preprocess_bwd(c, di, *saved, acc, g, st, (cfg->tuning & GS_TUNE_PBWD_2PHASE) ? 1 : 0, da, dm, cam);
         if (rc != GS_OK) return rc;
     }
     ctx->stats.kernel_launches += 2;  // k_composite_bwd, k_preprocess_bwd
     if (det && g.dL_dviewmatrix_z) ctx->stats.kernel_launches += 1;  // k_view_z_finalize
+    if (cam) ctx->stats.kernel_launches += 1;                        // k_camera_finalize
     return GS_OK;
 }
 }  // namespace
@@ -732,6 +747,13 @@ extern "C" int gs_backward_ex(GsContext *ctx, const GsConfig *cfg, const GsInput
                               const GsOutGrads *gout, const GsAlpha *alpha, const GsInGrads *gin, void *stream) {
     if (!alpha) return gs_set_error(GS_ERR_INVALID, "null alpha request");
     return backward(ctx, cfg, in, saved, gout, alpha->dL_dalpha, gin, stream);
+}
+
+extern "C" int gs_backward_cam(GsContext *ctx, const GsConfig *cfg, const GsInputs *in, const GsSaved *saved,
+                               const GsOutGrads *gout, const GsAlpha *alpha, const GsInGrads *gin, const GsCameraGrads *cam,
+                               void *stream) {
+    if (!cam) return gs_set_error(GS_ERR_INVALID, "null camera-gradient request");
+    return backward(ctx, cfg, in, saved, gout, alpha ? alpha->dL_dalpha : nullptr, gin, stream, cam);
 }
 
 extern "C" int gs_mark_visible(GsContext *ctx, const GsConfig *cfg, const float *means3D, uint8_t *present,

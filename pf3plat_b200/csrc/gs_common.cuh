@@ -146,9 +146,12 @@ int launch_composite_bwd(const DevCfg &c, const GsSaved &s, const float *dL_dcol
 // s.depth_mode != GS_DEPTH_Z: the depth gradient is chained through f'(z) (dm.near_far: the backward call's array)
 int launch_preprocess_bwd(const DevCfg &c, const DevInputs &in, const GsSaved &s, const float *grad_acc,
                           const GsInGrads &g, cudaStream_t st, int variant = 0 /* 1: the two-phase kernel (GS_TUNE_PBWD_2PHASE) */,
-                          const DetAcc &det = DetAcc{}, const DepthMode &dm = DepthMode{});
+                          const DetAcc &det = DetAcc{}, const DepthMode &dm = DepthMode{},
+                          const GsCameraGrads *cam = nullptr /* non-NULL: also the camera gradient */);
 // bytes of DetAcc::view_z for a configuration
 size_t det_view_z_bytes(const DevCfg &c);
+// bytes of DetAcc::view_z the camera gradient needs, in both modes: per-warp slots of 32 floats per view
+size_t camera_grad_scratch_bytes(const DevCfg &c);
 
 // per (view,Gaussian) accumulator written by the composite backward:
 //   0-2 dL/drgb, 3-4 dL/dmean2D (NDC-scaled), 5-7 dL/dconic (a, b stored once, c), 8 dL/dopacity, 9 dL/dz

@@ -119,9 +119,38 @@ __device__ __forceinline__ void sh_backward_band4(const float *sh, float *g4, co
     ddz += dz_;
 }
 
-// dL/d(view matrix entries 2, 6, 10, 14) of one view += the warp's sum of (gz * m, gz): a butterfly over the 32 lanes,
-// then one RED per component from lane 0.  Every lane of the warp must call it for the same view (inactive lanes with
-// zeros); the calls may sit at different points of the code (shfl.sync on sm_70 and later).
+// Per-view gradients (the depth channel's z column, the camera gradient) are sums over the Gaussians of a scene.  Each
+// warp adds up its lanes' terms with a butterfly over the 32 lanes.  Every lane of the warp must make the same sequence of
+// calls for the same view (inactive lanes with zeros); the calls may sit at different points of the code (shfl.sync on
+// sm_70 and later).
+template <int N>
+__device__ __forceinline__ void warp_sum(float (&x)[N]) {
+#pragma unroll
+    for (int off = 16; off > 0; off >>= 1) {
+#pragma unroll
+        for (int k = 0; k < N; k++) x[k] += __shfl_xor_sync(0xffffffffu, x[k], off);
+    }
+}
+
+// The warp's sum of x goes with plain stores to components [c0, c0 + N) of its own slot of slots[V][warps of the scene's
+// grid][NC], which a finalize kernel adds up in a fixed order: deterministic, and free of same-address atomics.
+// N, c0 and NC are multiples of 4.
+template <int NC, int N>
+__device__ __forceinline__ void view_partial(float *slots, int v, int c0, float (&x)[N]) {
+    static_assert(N % 4 == 0 && NC % 4 == 0, "slots are written in float4s");
+    warp_sum(x);
+    if ((threadIdx.x & 31) == 0) {
+        const size_t warps = (size_t)gridDim.x * (PB_THREADS / 32);
+        const size_t w = (size_t)blockIdx.x * (PB_THREADS / 32) + (threadIdx.x >> 5);
+        float4 *dst = reinterpret_cast<float4 *>(slots + ((size_t)v * warps + w) * NC + c0);
+#pragma unroll
+        for (int k = 0; k < N / 4; k++) dst[k] = make_float4(x[4 * k], x[4 * k + 1], x[4 * k + 2], x[4 * k + 3]);
+    }
+}
+
+// dL/d(view matrix entries 2, 6, 10, 14) of one view += the warp's sum of (gz * m, gz): warp_sum's butterfly written out
+// for four scalars (the array form allocates registers differently in the kernels that exist without the camera
+// gradient), then one RED per component from lane 0.  Same calling rules as warp_sum.
 __device__ __forceinline__ void red_view_z_grad(float *dst, float a, float b, float c, float d) {
 #pragma unroll
     for (int off = 16; off > 0; off >>= 1) {
@@ -139,7 +168,8 @@ __device__ __forceinline__ void red_view_z_grad(float *dst, float a, float b, fl
 }
 
 // Deterministic mode: the warp's sum goes to its own slot of det.view_z ([V][warps of the scene's grid][4]) with a
-// plain store, and k_view_z_finalize adds the slots up in warp order.  Same calling rules as red_view_z_grad.
+// plain store, as view_partial<4> would, and k_view_z_finalize adds the slots up in warp order.  This and
+// red_view_z_grad are warp_sum / view_partial written out for four scalars: the three must stay in step.
 template <bool DET>
 __device__ __forceinline__ void view_z_grad(const GsInGrads &g, const DetAcc &det, int v, float a, float b, float c,
                                             float d) {
@@ -159,6 +189,23 @@ __device__ __forceinline__ void view_z_grad(const GsInGrads &g, const DetAcc &de
     } else {
         red_view_z_grad(g.dL_dviewmatrix_z + (size_t)v * 4, a, b, c, d);
     }
+}
+
+// Camera gradient (GsCameraGrads): 27 terms per (view, Gaussian) pair in the slots of det.view_z, [V][warps][GS_CAM_NC]:
+//   0..11  dL/dviewmatrix[4k + r] at component 3k + r (k = 0..3, r = 0..2; the fourth column is never read)
+//   12..23 dL/dprojmatrix[4k + c] at component 12 + 3k + i, c = (0, 1, 3)[i] (the third column feeds no output)
+//   24..26 dL/dcampos, 27..31 zero (one component per lane of k_camera_finalize)
+// Each of the three groups is reduced where it is computed, which keeps few of the terms live at once.
+constexpr int GS_CAM_NC = 32;
+
+// the three partials of a pair that adds nothing (same calls as a visible pair makes)
+__device__ __forceinline__ void cam_partial_zero(float *slots, int v) {
+    float z12[12] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
+    view_partial<GS_CAM_NC>(slots, v, 0, z12);
+    float z12b[12] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
+    view_partial<GS_CAM_NC>(slots, v, 12, z12b);
+    float z8[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+    view_partial<GS_CAM_NC>(slots, v, 24, z8);
 }
 
 // VIEW_Z = 2 kernels: the depth channel carried f(z) of dm.mode, so the accumulated gz = sum alpha T dL/ddepth is dL/df,
@@ -192,7 +239,10 @@ __device__ __forceinline__ const float *load_det_acc(const DetAcc &det, size_t o
 // dL/do'.  rho is recomputed from the rebuilt 2-D covariance: dL/do = sum_v rho_v dL/do'_v, and o dL/do' drho/d(a0, b, c0)
 // joins dL/d(a, b, c) ahead of the cov2D -> cov3D and cov2D -> J -> mean chains (DESIGN.md 5.5).  The AA = false kernels
 // are the ones without it, instruction for instruction.
-template <bool HAS_SH, int MINB, int VIEW_Z = 0, bool DET = false, bool B4 = false, bool AA = false>
+// CAM: also the camera gradient (GsCameraGrads), into the slots of det.view_z (GS_CAM_NC components, in both modes), which
+// k_camera_finalize turns into dL/dviewmatrix, dL/dprojmatrix and dL/dcampos (DESIGN.md 5.5).  Never
+// with VIEW_Z = 1: the full gradient contains the z column.  The CAM = false kernels are the ones without it.
+template <bool HAS_SH, int MINB, int VIEW_Z = 0, bool DET = false, bool B4 = false, bool AA = false, bool CAM = false>
 __global__ void __launch_bounds__(PB_THREADS, MINB)
 k_preprocess_bwd(const DevCfg c, const DevInputs in, const uint8_t *__restrict__ meta, const float *__restrict__ acc,
                     const GsInGrads g, const DetAcc det, const DepthMode dm) {
@@ -270,6 +320,7 @@ k_preprocess_bwd(const DevCfg c, const DevInputs in, const uint8_t *__restrict__
         }
         if (!active) {
             if (VIEW_Z == 1 || (VIEW_Z == 2 && g.dL_dviewmatrix_z)) view_z_grad<DET>(g, det, v, 0.f, 0.f, 0.f, 0.f);
+            if constexpr (CAM) cam_partial_zero(det.view_z, v);
             continue;
         }
         const ViewCam &cam = sm->cams[vi % GS_CAM_CHUNK];
@@ -277,6 +328,9 @@ k_preprocess_bwd(const DevCfg c, const DevInputs in, const uint8_t *__restrict__
         const uint32_t mb = meta[o];
         float m2d[2] = {0.f, 0.f}, gcol[3] = {0.f, 0.f, 0.f};
         if ((VIEW_Z == 1 || (VIEW_Z == 2 && g.dL_dviewmatrix_z)) && !(mb & GS_META_VISIBLE)) view_z_grad<DET>(g, det, v, 0.f, 0.f, 0.f, 0.f);
+        if constexpr (CAM) {
+            if (!(mb & GS_META_VISIBLE)) cam_partial_zero(det.view_z, v);
+        }
         if (mb & GS_META_VISIBLE) {
             const float *a = acc + o * GS_ACC_STRIDE;
             float a_det[GS_ACC_STRIDE];
@@ -337,10 +391,12 @@ k_preprocess_bwd(const DevCfg c, const DevInputs in, const uint8_t *__restrict__
                                      2.0f * m1[1] * m1[2] * dL_dc);
                 }
                 float dJ00 = 0.f, dJ02 = 0.f, dJ11 = 0.f, dJ12 = 0.f;
+                float gw0[3], gw1[3];   // CAM: dL/d(rows of T = J W), kept for the view matrix's W
 #pragma unroll
                 for (int k = 0; k < 3; k++) {
                     const float gm0 = 2.0f * dL_da * s0[k] + dL_db * s1[k];
                     const float gm1 = 2.0f * dL_dc * s1[k] + dL_db * s0[k];
+                    if constexpr (CAM) { gw0[k] = gm0; gw1[k] = gm1; }
                     dJ00 += gm0 * cam.view[k * 4 + 0];
                     dJ02 += gm0 * cam.view[k * 4 + 2];
                     dJ11 += gm1 * cam.view[k * 4 + 1];
@@ -354,6 +410,21 @@ k_preprocess_bwd(const DevCfg c, const DevInputs in, const uint8_t *__restrict__
 #pragma unroll
                 for (int k = 0; k < 3; k++)
                     gm[k] += cam.view[k * 4 + 0] * dtx + cam.view[k * 4 + 1] * dty + cam.view[k * 4 + 2] * dtz;
+                if constexpr (CAM) {
+                    // t = W m + view[12..14]: dL/dview[4k + r] = dL/dt_r m_k, with the depth channel's gz on t.z; and
+                    // T = J W: dL/dW[r][k] = sum_i J[i][r] dL/dT[i][k] (J01 = J10 = 0)
+                    const float J00 = j.fx * tz, J11 = j.fy * tz, J02 = -j.fx * j.tx * tz2, J12 = -j.fy * j.ty * tz2;
+                    const float dt[3] = {dtx, dty, dtz + gz}, mk[3] = {m.x, m.y, m.z};
+                    float cv[12];
+#pragma unroll
+                    for (int k = 0; k < 3; k++) {
+                        cv[3 * k + 0] = dt[0] * mk[k] + J00 * gw0[k];
+                        cv[3 * k + 1] = dt[1] * mk[k] + J11 * gw1[k];
+                        cv[3 * k + 2] = dt[2] * mk[k] + J02 * gw0[k] + J12 * gw1[k];
+                    }
+                    cv[9] = dt[0]; cv[10] = dt[1]; cv[11] = dt[2];
+                    view_partial<GS_CAM_NC>(det.view_z, v, 0, cv);
+                }
             }
             // ---- mean2D (NDC units) -> mean through the perspective divide ----
             {
@@ -364,12 +435,26 @@ k_preprocess_bwd(const DevCfg c, const DevInputs in, const uint8_t *__restrict__
                 gm[0] += (pr[0] * mw - pr[3] * mul1) * m2d[0] + (pr[1] * mw - pr[3] * mul2) * m2d[1];
                 gm[1] += (pr[4] * mw - pr[7] * mul1) * m2d[0] + (pr[5] * mw - pr[7] * mul2) * m2d[1];
                 gm[2] += (pr[8] * mw - pr[11] * mul1) * m2d[0] + (pr[9] * mw - pr[11] * mul2) * m2d[1];
+                if constexpr (CAM) {
+                    // mh = Pf m + Pf[12..15]: dL/dPf[4k + c] = dL/dmh_c m_k for c = x, y, w (mh.z feeds no output)
+                    const float dmh[3] = {m2d[0] * mw, m2d[1] * mw, -(mul1 * m2d[0] + mul2 * m2d[1])};
+                    const float mk[3] = {m.x, m.y, m.z};
+                    float cp[12];
+#pragma unroll
+                    for (int k = 0; k < 3; k++) {
+#pragma unroll
+                        for (int i2 = 0; i2 < 3; i2++) cp[3 * k + i2] = dmh[i2] * mk[k];
+                    }
+                    cp[9] = dmh[0]; cp[10] = dmh[1]; cp[11] = dmh[2];
+                    view_partial<GS_CAM_NC>(det.view_z, v, 12, cp);
+                }
             }
             // ---- fused depth channel: z = (view * m).z ----
             gm[0] += cam.view[2] * gz;
             gm[1] += cam.view[6] * gz;
             gm[2] += cam.view[10] * gz;
             if (VIEW_Z == 1 || (VIEW_Z == 2 && g.dL_dviewmatrix_z)) view_z_grad<DET>(g, det, v, gz * m.x, gz * m.y, gz * m.z, gz);
+            float gcp[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};   // CAM: dL/dcampos = -dL/dd, d = m - campos
             // ---- colour -> SH coefficients and mean (view direction) ----
             if (HAS_SH) {
                 const float d[3] = {m.x - cam.campos[0], m.y - cam.campos[1], m.z - cam.campos[2]};
@@ -389,10 +474,16 @@ k_preprocess_bwd(const DevCfg c, const DevInputs in, const uint8_t *__restrict__
                 }
                 const float dot = d[0] * ddx + d[1] * ddy + d[2] * ddz;
                 const float inv3 = inv * inv * inv;
+                if constexpr (CAM) {
+                    gcp[0] = -(ddx * len2 - d[0] * dot) * inv3;
+                    gcp[1] = -(ddy * len2 - d[1] * dot) * inv3;
+                    gcp[2] = -(ddz * len2 - d[2] * dot) * inv3;
+                }
                 gm[0] += (ddx * len2 - d[0] * dot) * inv3;
                 gm[1] += (ddy * len2 - d[1] * dot) * inv3;
                 gm[2] += (ddz * len2 - d[2] * dot) * inv3;
             }
+            if constexpr (CAM) view_partial<GS_CAM_NC>(det.view_z, v, 24, gcp);
 #pragma unroll
             for (int k = 0; k < 3; k++) gmean[k] += s * gm[k];
         }
@@ -792,35 +883,39 @@ k_preprocess_bwd_2phase(const DevCfg c, const DevInputs in, const uint8_t *__res
     }
 }
 
-// AA: the anti-aliased kernels (single pass only: the two-phase kernel has none)
-template <int VIEW_Z, bool DET, bool AA>
+// AA: the anti-aliased kernels; CAM: the camera-gradient kernels (single pass only: the two-phase kernel has neither)
+template <int VIEW_Z, bool DET, bool AA, bool CAM>
 int launch_preprocess_bwd_t(const DevCfg &c, const DevInputs &in, const GsSaved &s, const float *grad_acc,
                             const GsInGrads &g, cudaStream_t st, int variant, const DetAcc &det, const DepthMode &dm) {
     dim3 grid((c.P + PB_THREADS - 1) / PB_THREADS, c.S);
     if (AA && variant == 1)
         return gs_set_error(GS_ERR_INVALID, "GS_TUNE_PBWD_2PHASE has no anti-aliased kernel (GS_FLAG_ANTIALIAS)");
+    if (CAM && variant == 1)
+        return gs_set_error(GS_ERR_INVALID, "GS_TUNE_PBWD_2PHASE has no camera-gradient kernel (GsCameraGrads)");
     if (in.shs && c.deg > 3) {   // degree 4: the single-pass kernel with band 4 compiled in
         if (variant == 1)
             return gs_set_error(GS_ERR_INVALID, "GS_TUNE_PBWD_2PHASE has no degree-4 kernel (sh_eval_max_degree = 4)");
         const size_t smem = PB_SMEM_HDR + (size_t)PB_THREADS * (c.M * 3 + PB_SH_B4) * 4;
-        auto kern = k_preprocess_bwd<true, PB_MIN_CTAS, VIEW_Z, DET, true, AA>;
+        auto kern = k_preprocess_bwd<true, PB_MIN_CTAS, VIEW_Z, DET, true, AA, CAM>;
         GS_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         kern<<<grid, PB_THREADS, smem, st>>>(c, in, s.meta, grad_acc, g, det, dm);
-    } else if (AA || variant != 1) {  // single pass over the views (default)
+    } else if (AA || CAM || variant != 1) {  // single pass over the views (default)
         if (in.shs) {
             size_t smem = PB_SMEM_HDR + (size_t)PB_THREADS * c.M * 12;
-            auto kern = k_preprocess_bwd<true, PB_MIN_CTAS, VIEW_Z, DET, false, AA>;
+            auto kern = k_preprocess_bwd<true, PB_MIN_CTAS, VIEW_Z, DET, false, AA, CAM>;
             GS_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
             kern<<<grid, PB_THREADS, smem, st>>>(c, in, s.meta, grad_acc, g, det, dm);
         } else {
-            k_preprocess_bwd<false, PB_MIN_CTAS, VIEW_Z, DET, false, AA><<<grid, PB_THREADS, PB_SMEM_HDR, st>>>(c, in, s.meta, grad_acc, g, det, dm);
+            k_preprocess_bwd<false, PB_MIN_CTAS, VIEW_Z, DET, false, AA, CAM><<<grid, PB_THREADS, PB_SMEM_HDR, st>>>(c, in, s.meta, grad_acc, g, det, dm);
         }
-    } else if (in.shs) {
-        size_t smem = PB_SMEM_HDR + (size_t)PB_THREADS * (c.M <= PB_SH_EVAL ? c.M * 3 : PB_SH_EVAL * 3 + 1) * 4;
-        GS_CUDA_OK(cudaFuncSetAttribute(k_preprocess_bwd_2phase<true, VIEW_Z, DET>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        k_preprocess_bwd_2phase<true, VIEW_Z, DET><<<grid, PB_THREADS, smem, st>>>(c, in, s.meta, grad_acc, g, det, dm);
-    } else {
-        k_preprocess_bwd_2phase<false, VIEW_Z, DET><<<grid, PB_THREADS, PB_SMEM_HDR, st>>>(c, in, s.meta, grad_acc, g, det, dm);
+    } else if constexpr (!CAM) {
+        if (in.shs) {
+            size_t smem = PB_SMEM_HDR + (size_t)PB_THREADS * (c.M <= PB_SH_EVAL ? c.M * 3 : PB_SH_EVAL * 3 + 1) * 4;
+            GS_CUDA_OK(cudaFuncSetAttribute(k_preprocess_bwd_2phase<true, VIEW_Z, DET>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            k_preprocess_bwd_2phase<true, VIEW_Z, DET><<<grid, PB_THREADS, smem, st>>>(c, in, s.meta, grad_acc, g, det, dm);
+        } else {
+            k_preprocess_bwd_2phase<false, VIEW_Z, DET><<<grid, PB_THREADS, PB_SMEM_HDR, st>>>(c, in, s.meta, grad_acc, g, det, dm);
+        }
     }
     GS_CUDA_OK(cudaGetLastError());
     return GS_OK;
@@ -837,36 +932,88 @@ __global__ void k_view_z_finalize(int V, int warps, const float *__restrict__ vi
     out[t] = sum;
 }
 
+// The camera gradient of view blockIdx.x from its per-warp slots [V][warps][GS_CAM_NC], written into GsCameraGrads in
+// its own layouts (zeros where an entry feeds nothing; a NULL output is skipped).  Fixed order, so deterministic: lane x
+// of row y adds component x of the slots w = y, y + 32, y + 64, ... in turn (each row reads whole 128-byte slots), then
+// row 0 adds the 32 row sums in row order.  One CTA of 32 x 32 threads per view: a view's slots are spread over 32
+// sequential chains instead of one (a scene of 500k Gaussians has 15 625 slots per view).
+__global__ void __launch_bounds__(1024) k_camera_finalize(int warps, const float *__restrict__ slots, GsCameraGrads out) {
+    __shared__ float part[32][33];
+    const int v = blockIdx.x, k = threadIdx.x, r = threadIdx.y;
+    const float *p = slots + (size_t)v * warps * GS_CAM_NC + k;
+    float sum = 0.f;
+    for (int w = r; w < warps; w += 32) sum += p[(size_t)w * GS_CAM_NC];
+    part[r][k] = sum;
+    __syncthreads();
+    if (r == 0) {
+        float t = 0.f;
+        for (int i = 0; i < 32; i++) t += part[i][k];
+        if (k < 12) {          // dL/dviewmatrix[4 (k / 3) + k % 3]
+            if (out.dL_dviewmatrix) out.dL_dviewmatrix[v * 16 + 4 * (k / 3) + k % 3] = t;
+        } else if (k < 24) {   // dL/dprojmatrix[4 i + (0, 1, 3)[j]], k - 12 = 3 i + j
+            const int i = (k - 12) / 3, j = (k - 12) % 3;
+            if (out.dL_dprojmatrix) out.dL_dprojmatrix[v * 16 + 4 * i + (j == 2 ? 3 : j)] = t;
+        } else if (k < 27) {
+            if (out.dL_dcampos) out.dL_dcampos[v * 3 + k - 24] = t;
+        }
+    } else if (r == 1 && k < 8) {   // the entries that feed nothing: the view matrix's 4th column, Pf's 3rd
+        if (k < 4 && out.dL_dviewmatrix) out.dL_dviewmatrix[v * 16 + 4 * k + 3] = 0.f;
+        if (k >= 4 && out.dL_dprojmatrix) out.dL_dprojmatrix[v * 16 + 4 * (k - 4) + 2] = 0.f;
+    }
+}
+
 int view_z_warps(const DevCfg &c) { return (c.P + PB_THREADS - 1) / PB_THREADS * (PB_THREADS / 32); }
 
-// the VIEW_Z kernels of one (DET, AA) pair: 2 after a forward whose depth channel carried f(z), else 1 when the view-matrix
-// gradient is wanted, else 0
-template <bool DET, bool AA>
+// the VIEW_Z kernels of one (DET, AA, CAM) triple: 2 after a forward whose depth channel carried f(z), else 1 when the
+// view matrix's z column is wanted (never with CAM), else 0
+template <bool DET, bool AA, bool CAM>
 int launch_preprocess_bwd_vz(const DevCfg &c, const DevInputs &in, const GsSaved &s, const float *grad_acc,
                              const GsInGrads &g, cudaStream_t st, int variant, const DetAcc &det, const DepthMode &dm) {
     const bool fz = (s.flags & GS_FLAG_DEPTH) && s.depth_mode != GS_DEPTH_Z;
-    if (fz) return launch_preprocess_bwd_t<2, DET, AA>(c, in, s, grad_acc, g, st, variant, det, dm);
-    return g.dL_dviewmatrix_z ? launch_preprocess_bwd_t<1, DET, AA>(c, in, s, grad_acc, g, st, variant, det, dm)
-                              : launch_preprocess_bwd_t<0, DET, AA>(c, in, s, grad_acc, g, st, variant, det, dm);
+    if (fz) return launch_preprocess_bwd_t<2, DET, AA, CAM>(c, in, s, grad_acc, g, st, variant, det, dm);
+    if constexpr (CAM) {
+        return launch_preprocess_bwd_t<0, DET, AA, true>(c, in, s, grad_acc, g, st, variant, det, dm);
+    } else {
+        return g.dL_dviewmatrix_z ? launch_preprocess_bwd_t<1, DET, AA, false>(c, in, s, grad_acc, g, st, variant, det, dm)
+                                  : launch_preprocess_bwd_t<0, DET, AA, false>(c, in, s, grad_acc, g, st, variant, det, dm);
+    }
+}
+
+template <bool CAM>
+int launch_preprocess_bwd_cam(const DevCfg &c, const DevInputs &in, const GsSaved &s, const float *grad_acc,
+                              const GsInGrads &g, cudaStream_t st, int variant, const DetAcc &det, const DepthMode &dm) {
+    // the forward's anti-aliasing setting, whatever this call's flags say
+    const bool aa = (s.flags & GS_FLAG_ANTIALIAS) != 0;
+    if (!det.acc)
+        return aa ? launch_preprocess_bwd_vz<false, true, CAM>(c, in, s, grad_acc, g, st, variant, det, dm)
+                  : launch_preprocess_bwd_vz<false, false, CAM>(c, in, s, grad_acc, g, st, variant, det, dm);
+    return aa ? launch_preprocess_bwd_vz<true, true, CAM>(c, in, s, grad_acc, g, st, variant, det, dm)
+              : launch_preprocess_bwd_vz<true, false, CAM>(c, in, s, grad_acc, g, st, variant, det, dm);
 }
 
 }  // namespace
 
 size_t det_view_z_bytes(const DevCfg &c) { return (size_t)c.V * view_z_warps(c) * 4 * sizeof(float); }
 
+size_t camera_grad_scratch_bytes(const DevCfg &c) { return (size_t)view_z_warps(c) * c.V * GS_CAM_NC * sizeof(float); }
+
 // g.dL_dviewmatrix_z non-NULL selects the VIEW_Z kernels; the caller has zeroed it (the kernels accumulate into it, or in
-// deterministic mode k_view_z_finalize writes it).  det.acc non-NULL selects the deterministic kernels.
+// deterministic mode k_view_z_finalize writes it).  det.acc non-NULL selects the deterministic kernels.  cam non-NULL
+// selects the camera-gradient kernels (never with dL_dviewmatrix_z): det.view_z then holds camera_grad_scratch_bytes of
+// per-warp slots, in both modes.
 int launch_preprocess_bwd(const DevCfg &c, const DevInputs &in, const GsSaved &s, const float *grad_acc,
-                          const GsInGrads &g, cudaStream_t st, int variant, const DetAcc &det, const DepthMode &dm) {
+                          const GsInGrads &g, cudaStream_t st, int variant, const DetAcc &det, const DepthMode &dm,
+                          const GsCameraGrads *cam) {
     if (c.P == 0) return GS_OK;
-    // the forward's anti-aliasing setting, whatever this call's flags say
-    const bool aa = (s.flags & GS_FLAG_ANTIALIAS) != 0;
-    if (!det.acc)
-        return aa ? launch_preprocess_bwd_vz<false, true>(c, in, s, grad_acc, g, st, variant, det, dm)
-                  : launch_preprocess_bwd_vz<false, false>(c, in, s, grad_acc, g, st, variant, det, dm);
-    const int rc = aa ? launch_preprocess_bwd_vz<true, true>(c, in, s, grad_acc, g, st, variant, det, dm)
-                      : launch_preprocess_bwd_vz<true, false>(c, in, s, grad_acc, g, st, variant, det, dm);
-    if (rc != GS_OK || !g.dL_dviewmatrix_z) return rc;
+    if (cam) {
+        const int rc = launch_preprocess_bwd_cam<true>(c, in, s, grad_acc, g, st, variant, det, dm);
+        if (rc != GS_OK) return rc;
+        k_camera_finalize<<<c.V, dim3(32, 32), 0, st>>>(view_z_warps(c), det.view_z, *cam);
+        GS_CUDA_OK(cudaGetLastError());
+        return GS_OK;
+    }
+    const int rc = launch_preprocess_bwd_cam<false>(c, in, s, grad_acc, g, st, variant, det, dm);
+    if (rc != GS_OK || !det.acc || !g.dL_dviewmatrix_z) return rc;
     k_view_z_finalize<<<(c.V * 4 + 127) / 128, 128, 0, st>>>(c.V, view_z_warps(c), det.view_z, g.dL_dviewmatrix_z);
     GS_CUDA_OK(cudaGetLastError());
     return GS_OK;

@@ -34,7 +34,7 @@ def render_views(extrinsics, intrinsics, near, far, image_shape, background_colo
                  gaussian_covariances, gaussian_sh_coefficients, gaussian_opacities, scale_invariant: bool = True,
                  use_sh: bool = True, with_depth: bool = False, sh_layout: str = "g_xyz_n",
                  sh_eval_max_degree: Optional[int] = None, depth_mode: str = "depth", with_alpha: bool = False,
-                 antialiasing: Optional[bool] = None):
+                 antialiasing: Optional[bool] = None, camera_gradients: Optional[bool] = None):
     """extrinsics (B,4,4) c2w, intrinsics (B,3,3), near/far (B,), background (B,3); Gaussians are per SCENE and NOT
     repeated per view: means (S,G,3), covariances (S,G,3,3) or (S,G,6), sh (S,G,3,d_sh) [or (S,G,d_sh,3) with
     sh_layout="g_n_xyz"], opacities (S,G); B % S == 0 and view b shows scene b // (B//S).
@@ -45,10 +45,16 @@ def render_views(extrinsics, intrinsics, near, far, image_shape, background_colo
     (cuda_splatting.py:245-251) at the UNSCALED camera-space depth z, with the unscaled near and far.
     with_alpha: also return the accumulated opacity alpha (B,h,w) = 1 - T_final, last: (color[, depth], alpha).
     antialiasing: the screen-space filter with opacity compensation (BatchSettings.antialiasing); None = the
-    process-wide setting (rasterizer.set_antialiasing, default off)."""
+    process-wide setting (rasterizer.set_antialiasing, default off).
+    camera_gradients: extrinsics that require grad get the full gradient of every output (colour, depth, alpha, the
+    anti-aliasing factor) through render_cuda's own camera glue (make_view_batch); None = the process-wide setting
+    (rasterizer.set_camera_gradients, default off: only the depth channel reaches them)."""
     assert use_sh or gaussian_sh_coefficients.shape[-1 if sh_layout == "g_xyz_n" else -2] == 1
     h, w = image_shape
-    vb = make_view_batch(extrinsics, intrinsics, near, far, scale_invariant)
+    if camera_gradients is None:
+        from .rasterizer import get_camera_gradients
+        camera_gradients = get_camera_gradients()
+    vb = make_view_batch(extrinsics, intrinsics, near, far, scale_invariant, camera_gradients)
     if sh_layout == "g_xyz_n":
         n = gaussian_sh_coefficients.shape[-1]
         shs = gaussian_sh_coefficients.transpose(-1, -2)  # (S,G,n,3); made contiguous by the operator
@@ -63,7 +69,7 @@ def render_views(extrinsics, intrinsics, near, far, image_shape, background_colo
                        view_scale=vb.scale if scale_invariant else None, with_depth=with_depth,
                        sh_eval_max_degree=sh_eval_max_degree, depth_mode=depth_mode,
                        depth_near_far=torch.stack([near, far], -1) if with_depth and depth_mode != "depth" else None,
-                       with_alpha=with_alpha, antialiasing=antialiasing)
+                       with_alpha=with_alpha, antialiasing=antialiasing, camera_gradients=bool(camera_gradients))
     B = extrinsics.shape[0]
     S = gaussian_means.shape[0]
     if use_sh:
@@ -89,7 +95,8 @@ def render_cuda(extrinsics, intrinsics, near, far, image_shape, background_color
 
 def decoder_forward(means, covariances, harmonics, opacities, extrinsics, intrinsics, near, far, image_shape,
                     background_color, depth_mode: Optional[str] = None, sh_eval_max_degree: Optional[int] = None,
-                    return_alpha: bool = False, antialiasing: Optional[bool] = None):
+                    return_alpha: bool = False, antialiasing: Optional[bool] = None,
+                    camera_gradients: Optional[bool] = None):
     """`DecoderSplattingCUDA.forward` (decoder_splatting_cuda.py:35-67) without the v-fold repeat: Gaussians
     (b,g,...), cameras (b,v,...).  Returns (color (b,v,3,h,w), depth (b,v,h,w) or None).  Every depth_mode of the
     reference ("depth", "disparity", "relative_disparity", "log") is composited in the same pass as the colour.
@@ -104,14 +111,17 @@ def decoder_forward(means, covariances, harmonics, opacities, extrinsics, intrin
     or not the extrinsics require grad.  sh_eval_max_degree: as render_views.
     return_alpha: also return the accumulated opacity (b,v,h,w) = 1 - T_final of the same pass, as (color, depth, alpha)
     (depth None without a depth_mode).  It trains the Gaussians' geometry and opacities, never the extrinsics.
-    antialiasing: as render_views; the opacity compensation gives the extrinsics no gradient either."""
+    antialiasing: as render_views; the opacity compensation gives the extrinsics no gradient either.
+    camera_gradients (None = rasterizer.get_camera_gradients(), default off): the extrinsics get the full gradient of
+    every output instead -- colour, depth (the z-column route above is then part of it, not added again), alpha and
+    the anti-aliasing factor -- for photometric pose training and test-time pose refinement."""
     b, v = extrinsics.shape[:2]
     flat = lambda t: t.reshape(b * v, *t.shape[2:])
     bg = background_color.reshape(1, 3).expand(b * v, 3)
     out = render_views(flat(extrinsics), flat(intrinsics), flat(near), flat(far), image_shape, bg, means,
                        covariances, harmonics, opacities, with_depth=depth_mode is not None,
                        sh_eval_max_degree=sh_eval_max_degree, depth_mode=depth_mode or "depth", with_alpha=return_alpha,
-                       antialiasing=antialiasing)
+                       antialiasing=antialiasing, camera_gradients=camera_gradients)
     alpha = None
     if return_alpha:
         *out, alpha = out

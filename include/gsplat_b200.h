@@ -416,6 +416,45 @@ GS_API int gs_photometric_backward(const GsLossConfig *cfg, const float *predict
                                    float *dL_dground_truth, void *scratch, void *stream);
 
 /*
+ * Pose (correspondence) loss = PF3plat's Losspose (src/loss/loss_pose.py:29-129), per segment s = (scene, pair (a, c)),
+ * segments scene-major and pairs in the reference's order [(a, c) for a in range(views) for c in range(a + 1, views)]:
+ *   L3[s] = conf[s] sum_n (w_n / max(sum |w|, 1e-12)) |R_s xyz_a(p) + t_s - xyz_c(q)|
+ *   L2[s] = sum_n huber_0.01(|project_s(p, d_a(p)) - xy(q)|) / 0.01
+ * with p = id_a[n], q = id_c[n] flat pixel indices of views a and c of the segment's scene (DESIGN.md 5.12).  The
+ * caller forms weight_3d mean(L3) + weight_2d mean(L2).  Device pointers: T [S,16] row-major (c2w[c] or
+ * c2w[c] @ inverse(c2w[a])), kinv_a [S,9] (K_a^-1), k_c [S,9], conf [S], seg [S,3] (scene, a, c), offsets [S+1] into
+ * the matches (CSR), id_a / id_c int64 [matches], w [matches], depth [batch*views, h, w], xyz [batch, views, 3, h, w].
+ * Gradients are written (not accumulated): dL_dT [S,16], dL_ddepth and dL_dxyz shaped as their inputs, dL_dw
+ * [matches], dL_dconf [S]; any may be NULL.  The incoming dL_dL3 / dL_dL2 [S] are device arrays (NULL = zero).  An index
+ * outside [0, h w) is never read: its segment's L3, L2 and gradient terms are NaN.  Non-finite depth at an unmatched
+ * source pixel makes dL_ddepth there and dL_dT of its pairs NaN, as the reference's dense projection does.  Scratch:
+ * gs_pose_loss_scratch_bytes(cfg), 256-byte aligned, needed only for dL_ddepth / dL_dxyz.  Deterministic (no float
+ * atomics), no host synchronisation.
+ */
+typedef struct GsPoseLossConfig {
+    int32_t batch, views, height, width;
+    int32_t segments, reserved_; /* segments = batch * views (views - 1) / 2 */
+    int64_t matches;             /* total over all segments = offsets[S] */
+} GsPoseLossConfig;
+
+typedef struct GsPoseLossInputs {
+    const float *T, *kinv_a, *k_c, *conf;
+    const int32_t *seg;
+    const int64_t *offsets, *id_a, *id_c;
+    const float *w, *depth, *xyz;
+} GsPoseLossInputs;
+
+typedef struct GsPoseLossGrads {
+    float *dL_dT, *dL_ddepth, *dL_dxyz, *dL_dw, *dL_dconf;
+} GsPoseLossGrads;
+
+GS_API int64_t gs_pose_loss_scratch_bytes(const GsPoseLossConfig *cfg); /* -1 for an invalid config */
+GS_API int gs_pose_loss_forward(const GsPoseLossConfig *cfg, const GsPoseLossInputs *in, float *out_L3, float *out_L2,
+                                void *stream);
+GS_API int gs_pose_loss_backward(const GsPoseLossConfig *cfg, const GsPoseLossInputs *in, const float *dL_dL3,
+                                 const float *dL_dL2, const GsPoseLossGrads *grads, void *scratch, void *stream);
+
+/*
  * LPIPS-VGG = the `lpips` package's LPIPS(net="vgg", version="0.1"), spatial=False, as PF3plat's LossLpips
  * (src/loss/loss_lpips.py:55-59) and compute_lpips (src/evaluation/metrics.py:27-33) call it; forward and input
  * gradients (the weights are constants).  The weights are an input:

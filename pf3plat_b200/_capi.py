@@ -138,6 +138,20 @@ class GsLpipsConfig(Structure):
 GsLpipsConfig.reserved_ = GsLpipsConfig.precision  # the header's other name for the field (a union member)
 
 
+class GsPoseLossConfig(Structure):
+    _fields_ = [("batch", c_int32), ("views", c_int32), ("height", c_int32), ("width", c_int32),
+                ("segments", c_int32), ("reserved_", c_int32), ("matches", c_int64)]
+
+
+class GsPoseLossInputs(Structure):
+    _fields_ = [(n, c_void_p) for n in ("T", "kinv_a", "k_c", "conf", "seg", "offsets", "id_a", "id_c", "w", "depth",
+                                        "xyz")]
+
+
+class GsPoseLossGrads(Structure):
+    _fields_ = [(n, c_void_p) for n in ("dL_dT", "dL_ddepth", "dL_dxyz", "dL_dw", "dL_dconf")]
+
+
 SYMBOLS = {
     "gs_abi_version": (c_int, []),
     "gs_last_error": (c_char_p, []),
@@ -182,6 +196,10 @@ SYMBOLS = {
     "gs_lpips_workspace_bytes": (c_int64, [POINTER(GsLpipsConfig)]),
     "gs_lpips_forward": (c_int, [c_void_p, POINTER(GsLpipsConfig), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "gs_lpips_backward": (c_int, [c_void_p, POINTER(GsLpipsConfig), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "gs_pose_loss_scratch_bytes": (c_int64, [POINTER(GsPoseLossConfig)]),
+    "gs_pose_loss_forward": (c_int, [POINTER(GsPoseLossConfig), POINTER(GsPoseLossInputs), c_void_p, c_void_p, c_void_p]),
+    "gs_pose_loss_backward": (c_int, [POINTER(GsPoseLossConfig), POINTER(GsPoseLossInputs), c_void_p, c_void_p,
+                                      POINTER(GsPoseLossGrads), c_void_p, c_void_p]),
 }
 
 

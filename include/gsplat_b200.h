@@ -88,6 +88,7 @@ enum {
     GS_TUNE_PRE_SH_RAW16 = 65536u,    /* preprocess, M > 16, device-resident SH: stage 16-byte pieces at the rows' own stride (what the zero-copy feed of gs_render_host uses) instead of gathering the 16 evaluated coefficients with 4-byte copies into compacted rows (A/B: 0.246 vs 0.220 ms on C2) */
     GS_TUNE_NO_ZERO_COPY = 131072u,   /* gs_render_host: always upload the SH block with the copy engine (in pieces) even when the caller's buffer is pinned and preprocess could pull it over PCIe itself (A/B) */
     GS_TUNE_NO_SPLIT_COLOUR = 262144u, /* gs_render_host, zero-copy feed: one fused preprocess pulling the SH block instead of geometry + tile sort on the launch stream with k_sh_colour pulling the block on a second stream (A/B) */
+    GS_TUNE_ALL_STRATA = 524288u,     /* per-view stratified binning: the stratum sort sorts every stratum of every tile instead of those the tile's previous forward reached (+1); the reference of the lazily sorted lists (A/B) */
     GS_TUNE_FEED_PIECES_SHIFT = 8     /* gs_render_host: bits 8..11 = pieces the SH block is copied in (0 default, 1 = one plain copy) */
 };
 

@@ -41,6 +41,7 @@ GS_TUNE_DIRECT_OUTPUT = 32768
 GS_TUNE_PRE_SH_RAW16 = 65536
 GS_TUNE_NO_ZERO_COPY = 131072
 GS_TUNE_NO_SPLIT_COLOUR = 262144
+GS_TUNE_ALL_STRATA = 524288
 GS_TUNE_FEED_PIECES_SHIFT = 8
 GS_NUM_STAGES = 8
 STAGE_NAMES = ("preprocess", "bin_scan", "bin_emit", "bin_sort", "composite", "composite_bwd", "preprocess_bwd", "sh_colour")

@@ -13,6 +13,10 @@ constexpr uint32_t BIN_STRATUM_CAP = 2048;  // longest sub-bucket k_stratum_sort
 // Bigger bucket sets are filled by the view-major k_emit_buckets: appends from preprocess touch all views' buckets, far
 // beyond L2 as partial-sector DRAM writes.  C2's (above the 50 MB L2) still fill faster from preprocess on an H100 (README.md).
 constexpr size_t BIN_FUSED_EMIT_MAX_BYTES = (size_t)96 << 20;
+// Lazy strata: k_composite_fwd sorts a stratum the stratum sort skipped in its record stage (2 x 256 x 48 bytes), as
+// 8-byte keys.  A shape whose sub-buckets do not fit it sorts every stratum up front.
+constexpr size_t BIN_LAZY_STAGE_BYTES = 2 * 256 * 48;
+inline bool lazy_stratum_fits(uint32_t sub_cap) { return (size_t)sub_cap * 8 <= BIN_LAZY_STAGE_BYTES; }
 
 enum { STRATA_UNKNOWN = 0, STRATA_TRIAL = 1, STRATA_ON = 2, STRATA_OFF = 3 };
 
@@ -25,6 +29,9 @@ struct SpecState {
     // Gaussians on a smooth surface), so boundaries are learned per (view, tile) from the exact call's sorted lists and
     // refreshed by every stratum sort: two tables, tile_tab the one to read, swapped on success
     int per_tile = 0, tile_tab = 0;
+    // the shape's "strata needed" table (one byte per (view, tile): how many of the tile's strata its last forward read)
+    // holds what a committed lazy forward wrote; otherwise it must be reset to BIN_SUB (sort everything) before use
+    bool need_learned = false;
 };
 
 // A context remembers a few shapes (views, tiles, Gaussians per scene, scenes), so a caller that alternates shapes --
@@ -65,6 +72,9 @@ struct BinPlan {
     int read_tab = -1;         // boundary table the emission reads (index into the slot's tables; -1: none)
     int write_tab = -1;        // table the stratum sort writes the next call's boundaries into (-1: none)
     bool fused_emit = false;   // preprocess appends to the buckets itself (else k_emit_buckets)
+    // per-view strata with the rank sort: the stratum sort sorts only the strata the tile's last forward needed, the
+    // compositor sorts any further one it reaches and records what this call needed; reset_need: the table is stale
+    bool lazy_strata = false, reset_need = false;
 };
 
 inline BinPlan plan_binning(const SpecState &s, const BinShape &sh, size_t n, bool have_table, uint32_t tuning) {
@@ -87,6 +97,11 @@ inline BinPlan plan_binning(const SpecState &s, const BinShape &sh, size_t n, bo
     if (p.strata) p.read_tab = p.per_tile ? s.tile_tab : 0;
     if (p.strata && p.per_tile) p.write_tab = s.tile_tab ^ 1;
     p.fused_emit = slots * p.sub_cap * 8 <= BIN_FUSED_EMIT_MAX_BYTES && !(tuning & GS_TUNE_SEPARATE_EMIT);
+    // per-tile boundaries are refreshed by the stratum sort from every position of the list, the merge sort and the
+    // warp-specialised compositor have no lazy counterpart
+    p.lazy_strata = p.strata && !p.per_tile && lazy_stratum_fits(p.sub_cap) &&
+                    !(tuning & (GS_TUNE_ALL_STRATA | GS_TUNE_STRATA_MERGE_SORT | GS_TUNE_FWD_WS));
+    p.reset_need = p.lazy_strata && !s.need_learned;
     return p;
 }
 
@@ -115,6 +130,7 @@ inline void learn_capacities(SpecState &s, const BinShape &sh, uint32_t max_tile
 inline bool learn_speculative(SpecState &s, const BinShape &sh, const BinPlan &p, const uint32_t *words, size_t sort_bytes,
                               uint32_t tuning, bool *release_sort) {
     *release_sort = false;
+    s.need_learned = p.lazy_strata && words[3] == 0;  // an overflowed call's compositor read clamped lists
     if (words[3] != 0) {
         s.sub_cap = 0;
         if (p.strata) {
@@ -152,6 +168,7 @@ enum { LEARN_NONE = 0, LEARN_PER_VIEW = 1, LEARN_PER_TILE = 2 };
 
 inline int learn_exact(SpecState &s, const BinShape &sh, size_t n, uint32_t max_tile, uint32_t max_sub, bool smem_sort,
                        uint32_t tuning) {
+    s.need_learned = false;
     learn_capacities(s, sh, max_tile, max_sub);
     if (!(smem_sort && s.sub_cap > 0 && s.strata_state != STRATA_OFF && !(tuning & GS_TUNE_NO_STRATA) && n > 0))
         return LEARN_NONE;

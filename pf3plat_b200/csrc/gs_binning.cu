@@ -549,12 +549,17 @@ __global__ void __launch_bounds__(RS_WARPS * 32)
 k_stratum_rank_sort(uint32_t nvt, uint32_t sub_cap, uint32_t cap_pad, const uint32_t *__restrict__ cursor,
                     const uint64_t *__restrict__ bucket, uint32_t *__restrict__ point_list, uint2 *__restrict__ ranges,
                     uint32_t *__restrict__ acc, uint32_t *__restrict__ info, const float4 *__restrict__ rec2, uint32_t P,
-                    uint32_t ntiles, float *__restrict__ next) {
+                    uint32_t ntiles, float *__restrict__ next, const uint8_t *__restrict__ need) {
     extern __shared__ __align__(16) unsigned char rs_smem[];
     const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const uint32_t sidx = blockIdx.x * RS_WARPS + warp;   // (view, tile, stratum)
     if (sidx >= nvt * BIN_SUB) return;
     const uint32_t vt = sidx / BIN_SUB, k = sidx % BIN_SUB;
+    // lazy strata: the strata the tile's previous forward read; the compositor sorts the rest if it gets there (a margin
+    // of one more stratum, for a moving cloud, was slower on C2 and on the moving cloud alike: DESIGN.md 5.2).  Stratum 0
+    // is always sorted: its warp also accounts for the tile in the verdict.
+    const uint32_t sorted = need ? min(max((uint32_t)need[vt], 1u), (uint32_t)BIN_SUB) : (uint32_t)BIN_SUB;
+    if (k >= sorted) return;
     // the tile's eight cursors: clamped counts, this stratum's offset inside the tile's list, the verdict's sums
     const uint32_t raw = lane < BIN_SUB ? cursor[((size_t)vt * BIN_SUB + lane) * BIN_PAD] : 0u;
     const uint32_t cnt = min(raw, sub_cap);  // clamped: an overflowed call is redone
@@ -564,8 +569,9 @@ k_stratum_rank_sort(uint32_t nvt, uint32_t sub_cap, uint32_t cap_pad, const uint
     const uint32_t base = vt * BIN_SUB * sub_cap;
     if (k == 0) {
         const uint32_t raw_total = __reduce_add_sync(0xffffffffu, raw), raw_max = __reduce_max_sync(0xffffffffu, raw);
+        const uint32_t prefix = __reduce_add_sync(0xffffffffu, lane < sorted ? cnt : 0u);  // the sorted strata, in order
         if (lane == 0) {
-            ranges[vt] = make_uint2(base, base + total);
+            ranges[vt] = make_uint2(base, base + prefix);
             if (atomicAdd(&acc[0], raw_total) + raw_total < raw_total) atomicOr(&acc[3], 1u);  // 32-bit wrap: redo exactly
             atomicMax(&acc[1], raw_total);
             atomicMax(&acc[2], raw_max);
@@ -735,7 +741,7 @@ int launch_stratum_sort(int nvt, uint32_t sub_cap, const uint32_t *cursor, const
 
 int bin_sort_strata(const DevCfg &c, uint32_t sub_cap, const uint32_t *cursor, const void *bucket, uint32_t *point_list,
                     uint2 *ranges, uint32_t *acc, uint32_t *info, cudaStream_t st, bool merge_sort, const float4 *rec2,
-                    float *next_tile_strata) {
+                    float *next_tile_strata, const uint8_t *need) {
     if (!merge_sort || next_tile_strata) {   // (the merge-sort kernel does not refresh per-tile boundaries)
         // hand-written warp-per-stratum distribution sort (default)
         if (sub_cap > BIN_STRATUM_CAP) return gs_set_error(GS_ERR_INVALID, "stratum capacity beyond the sort's");
@@ -747,7 +753,7 @@ int bin_sort_strata(const DevCfg &c, uint32_t sub_cap, const uint32_t *cursor, c
         const uint32_t ctas = (nvt * BIN_SUB + RS_WARPS - 1) / RS_WARPS;
         k_stratum_rank_sort<<<ctas, RS_WARPS * 32, smem, st>>>(nvt, sub_cap, cap_pad, cursor, static_cast<const uint64_t *>(bucket),
                                                                point_list, ranges, acc, info, rec2, (uint32_t)c.P, (uint32_t)c.ntiles,
-                                                               next_tile_strata);
+                                                               next_tile_strata, need);
         GS_CUDA_OK(cudaGetLastError());
         return GS_OK;
     }
@@ -767,7 +773,11 @@ int bin_sort_strata(const DevCfg &c, uint32_t sub_cap, const uint32_t *cursor, c
 size_t bin_strata_bytes(const DevCfg &c) {
     const size_t per_view = (size_t)c.V * BIN_SUB * 4 + (size_t)c.V * STRATA_BINS * 4;
     const size_t per_tile = 2 * (size_t)c.V * c.ntiles * BIN_SUB * 4;  // two tables: this call's and the next one's
-    return per_view > per_tile ? per_view : per_tile;
+    return align256(per_view > per_tile ? per_view : per_tile) + (size_t)c.V * c.ntiles;
+}
+
+uint8_t *bin_need_table(const DevCfg &c, void *strata_buf) {
+    return static_cast<uint8_t *>(strata_buf) + bin_strata_bytes(c) - (size_t)c.V * c.ntiles;
 }
 
 int bin_learn_strata(const DevCfg &c, const ushort4 *rects, const float4 *rec2, void *strata_buf, cudaStream_t st) {

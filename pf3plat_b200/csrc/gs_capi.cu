@@ -361,6 +361,7 @@ struct FwdCall {
     size_t ctr_bytes;
     GsSaved *s;
     bool colour_pending;   // k_sh_colour is (or may still be) writing into s->rec1 / s->rec2 on the aux stream
+    LazyStrata lazy;       // speculative call with lazy strata: what the compositor needs to sort the skipped strata
     int64_t D;
     size_t list_bytes;
     int start_colour();
@@ -408,7 +409,7 @@ struct FwdCall {
             colour_pending = false;
             FWD_CUDA(cudaStreamWaitEvent(st, ctx->ev_colour, 0), "cudaStreamWaitEvent(colour)");
         }
-        return timed(GS_STAGE_COMPOSITE, [&] { return launch_composite_fwd(c, *s, out->color, out->depth, st, composite_variant, alpha); });
+        return timed(GS_STAGE_COMPOSITE, [&] { return launch_composite_fwd(c, *s, out->color, out->depth, st, composite_variant, alpha, lazy); });
     }
 };
 
@@ -479,8 +480,13 @@ int FwdCall::speculate(SpecState &spec, const BinShape &shape, const BinPlan &pl
     {
         StageTimer t(ctx, GS_STAGE_BIN_SORT, st);
         if (plan.strata) {
+            // lazy strata: one table per shape is enough -- this call's sort reads it before its compositor rewrites it
+            uint8_t *need = plan.lazy_strata ? bin_need_table(c, tabs.p) : nullptr;
+            if (plan.reset_need)
+                FWD_CUDA(cudaMemsetAsync(need, BIN_SUB, (size_t)c.V * c.ntiles, st), "cudaMemsetAsync(need)");
+            if (need) lazy = LazyStrata{cursor, static_cast<const uint64_t *>(ctx->sort.p), plan.sub_cap, need};
             FWD_OK(bin_sort_strata(c, plan.sub_cap, cursor, ctx->sort.p, s->point_list, s->ranges, verdict_acc,
-                                   ctx->d_word, st, merge_sort, s->rec2, strata_next));
+                                   ctx->d_word, st, merge_sort, s->rec2, strata_next, need));
             FWD_CUDA(cudaEventRecord(ctx->ev_info, st), "read back binning info");
             FWD_OK(start_radii_copy());
         } else {

@@ -109,12 +109,14 @@ int bin_spec_check(const DevCfg &c, uint32_t sub_cap, uint32_t tile_limit, const
 int bin_sort_strata(const DevCfg &c, uint32_t sub_cap, const uint32_t *cursor, const void *bucket, uint32_t *point_list,
                     uint2 *ranges, uint32_t *acc /* 8 zeroed words */, uint32_t *info, cudaStream_t st,
                     bool merge_sort = false /* the round-1 cub::BlockMergeSort kernel (GS_TUNE_STRATA_MERGE_SORT) */,
-                    const float4 *rec2 = nullptr, float *next_tile_strata = nullptr /* per-tile mode: boundaries of the next call */);
+                    const float4 *rec2 = nullptr, float *next_tile_strata = nullptr /* per-tile mode: boundaries of the next call */,
+                    const uint8_t *need = nullptr /* lazy strata: sort strata k <= need[vt] only (NULL: all) */);
 // per-(view, tile) stratum boundaries from the sorted lists of an exact-path call
 int bin_learn_tile_strata(const DevCfg &c, const uint32_t *point_list, const uint2 *ranges, const float4 *rec2, float *table,
                           cudaStream_t st);
 // depth strata: per-view octiles of the depths of the binned Gaussians (weighted by their tile count), for the NEXT call
-size_t bin_strata_bytes(const DevCfg &c);          // strata table [V][BIN_SUB] floats + histogram scratch
+size_t bin_strata_bytes(const DevCfg &c);          // strata table [V][BIN_SUB] floats + histogram scratch + need table
+uint8_t *bin_need_table(const DevCfg &c, void *strata_buf);  // lazy strata: [V * ntiles] strata each tile's last forward read
 int bin_learn_strata(const DevCfg &c, const ushort4 *rects, const float4 *rec2, void *strata_buf, cudaStream_t st);
 int bin_sort_spec(const DevCfg &c, uint32_t sub_cap, uint32_t tile_limit, const uint32_t *cursor, const void *bucket,
                   uint32_t *point_list, uint2 *ranges, cudaStream_t st);
@@ -135,9 +137,18 @@ struct DetAcc {
 // compositors take the same word for the depth term of dL/dalpha
 // alpha (GsAlpha): the forward also writes 1 - T_final per pixel ([V*H*W]); the backward takes dL/dalpha into the
 // background term of every dL/dalpha_i.  NULL: the kernels of before.
+// Lazy strata (DESIGN.md 5.2): ranges[vt] covers the sorted strata only; a tile whose pixels are not all saturated at its
+// end sorts the next stratum from its sub-bucket into place, extends ranges[vt].y, and records in need[vt] how many
+// strata it read.  cursor == NULL: the lists are sorted whole.
+struct LazyStrata {
+    const uint32_t *cursor;   // the sub-buckets' counts (BIN_PAD stride; clamped to sub_cap)
+    const uint64_t *bucket;   // (depth bits << 32 | index) keys, sub-bucket (vt * BIN_SUB + k) at its * sub_cap
+    uint32_t sub_cap;
+    uint8_t *need;            // [V * ntiles]
+};
 int launch_composite_fwd(const DevCfg &c, const GsSaved &s, float *color, float *depth, cudaStream_t st,
                          int variant = 0 /* 2: the persistent warp-specialised kernel (GS_TUNE_FWD_WS) */,
-                         float *alpha = nullptr);
+                         float *alpha = nullptr, const LazyStrata &lazy = LazyStrata{});
 int launch_composite_bwd(const DevCfg &c, const GsSaved &s, const float *dL_dcolor, const float *dL_ddepth,
                          float *grad_acc /* [V*P*GS_ACC_STRIDE], zeroed */, cudaStream_t st,
                          int variant = 0 /* 1: the round-1 kernel (GS_TUNE_BWD_V1) */,

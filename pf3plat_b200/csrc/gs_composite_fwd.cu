@@ -20,6 +20,8 @@
 // pipeline over groups of views (k_tile_sort of group g+1 on a side stream under the compositing of group g):
 // slower than serial on C2 -- the co-resident sort CTAs take registers/shared memory from the
 // compositor without filling its idle issue slots.
+#include <type_traits>
+
 #include "gs_common.cuh"
 
 namespace {
@@ -32,16 +34,75 @@ constexpr int CF_BATCH = 256;
 struct CfStage {
     float4 rec[CF_BATCH][3];
 };
+static_assert(2 * sizeof(CfStage) == BIN_LAZY_STAGE_BYTES, "the lazy stratum sort's keys live in the stage");
+
+// Lazy strata, off the compositing path (own frames, so the main loop keeps its registers).
+// The tile's next non-empty stratum -- the one whose entries start at list position `sorted` -- is sorted by the whole
+// CTA into its final place: its keys into the stage, every key ranked against all of them (keys are unique: depth bits,
+// index), its index stored at its rank.  Returns the stratum's length (0: the list is complete).
+__device__ __noinline__ uint32_t lazy_sort_next(const LazyStrata lz, uint32_t vt, uint32_t sorted, uint64_t *keys,
+                                                uint32_t *list /* the tile's list */) {
+    __shared__ uint32_t s_k, s_n;
+    if (threadIdx.x == 0) {
+        uint32_t below = 0, kk = BIN_SUB, nn = 0;
+        for (uint32_t k = 0; k < BIN_SUB; k++) {
+            const uint32_t cnt = min(lz.cursor[((size_t)vt * BIN_SUB + k) * BIN_PAD], lz.sub_cap);
+            if (below >= sorted && cnt > 0) {  // (the sorted prefix always ends on a stratum boundary)
+                kk = k;
+                nn = cnt;
+                break;
+            }
+            below += cnt;
+        }
+        s_k = kk;
+        s_n = nn;
+    }
+    __syncthreads();
+    const uint32_t k = s_k, n = s_n;
+    if (n == 0) return 0;
+    const uint64_t *src = lz.bucket + ((size_t)vt * BIN_SUB + k) * lz.sub_cap;
+    for (uint32_t i = threadIdx.x; i < n; i += CF_THREADS) keys[i] = src[i];
+    __syncthreads();
+    for (uint32_t i = threadIdx.x; i < n; i += CF_THREADS) {
+        const uint64_t key = keys[i];
+        uint32_t rank = 0;
+        for (uint32_t j = 0; j < n; j++) rank += keys[j] < key ? 1u : 0u;
+        list[sorted + rank] = (uint32_t)key;
+    }
+    __syncthreads();  // the entries are visible to the whole CTA, and the stage is free again
+    return n;
+}
+
+// Lazy strata, when the CTA retires (thread 0): the list's sorted length goes to ranges[vt].y (every later reader of the
+// list sees the entries sorted here), and need[vt] = 1 + the stratum of list position `reach` (1-based; 0: none), which
+// lies at or a chunk behind the entry that saturated the tile's last pixel, or BIN_SUB when a pixel is not saturated.
+__device__ __noinline__ void lazy_record(const LazyStrata lz, uint32_t vt, uint32_t reach, bool all_done, uint2 *range,
+                                         uint32_t sorted) {
+    uint32_t need = BIN_SUB;
+    if (all_done) {
+        uint32_t below = 0;
+        need = 1;
+        for (uint32_t k = 0; k + 1 < BIN_SUB; k++) {
+            below += min(lz.cursor[((size_t)vt * BIN_SUB + k) * BIN_PAD], lz.sub_cap);
+            need += reach > 0 && below < reach ? 1u : 0u;  // the entry at 0-based position reach - 1 lies past stratum k
+        }
+    }
+    lz.need[vt] = (uint8_t)need;
+    range->y = range->x + sorted;
+}
 
 // DEPTH: 0 no depth channel; 1 the channel composites rec2.y (GS_DEPTH_Z); 2 it composites rec2.w, the f(z) preprocess
 // stored for the other depth modes.  Values 0 and 1 are the kernels of before, instruction for instruction.
 // ALPHA: also store the accumulated opacity 1 - T next to final_T (GsAlpha); false is the kernel of before.
-template <int DEPTH, int MINB, bool ALPHA = false>
+// LAZY: lazy strata (`lazy`): past the end of the sorted prefix the CTA sorts the next stratum and composites it as a list
+// of its own; false is the kernel of before.
+template <int DEPTH, int MINB, bool ALPHA = false, bool LAZY = false>
 __global__ void __launch_bounds__(CF_THREADS, MINB)
 k_composite_fwd(const DevCfg c, const float4 *__restrict__ rec0, const float4 *__restrict__ rec1,
                 const float4 *__restrict__ rec2, const uint32_t *__restrict__ point_list,
-                const uint2 *__restrict__ ranges, float *__restrict__ color, float *__restrict__ depth,
-                float *__restrict__ final_T, uint32_t *__restrict__ n_contrib, float *__restrict__ alpha_out) {
+                uint2 *__restrict__ ranges, float *__restrict__ color, float *__restrict__ depth,
+                float *__restrict__ final_T, uint32_t *__restrict__ n_contrib, float *__restrict__ alpha_out,
+                const LazyStrata lazy) {
     __shared__ CfStage stage[2];
 
     const int v = blockIdx.y;
@@ -54,9 +115,10 @@ k_composite_fwd(const DevCfg c, const float4 *__restrict__ rec0, const float4 *_
     const float pxf = (float)px, pyf = (float)py;
     const float bx0 = (float)bx, bx1 = (float)(bx + 7), by0 = (float)by, by1 = (float)(by + 3);
 
-    const uint2 range = ranges[(size_t)v * c.ntiles + tile];
-    const uint32_t total = range.y - range.x;
-    const uint32_t nbatches = (total + CF_BATCH - 1) / CF_BATCH;
+    const uint32_t vt = (uint32_t)v * (uint32_t)c.ntiles + (uint32_t)tile;
+    const uint2 range = ranges[vt];
+    // the list composited below: `total` entries from point_list[lbase] on (LAZY: then each stratum sorted here)
+    uint32_t lbase = range.x, total = range.y - range.x;
     const size_t rbase = (size_t)v * c.P;
     const uint32_t stage_addr = smem_u32(&stage[0].rec[0][0]);
 
@@ -71,16 +133,27 @@ k_composite_fwd(const DevCfg c, const float4 *__restrict__ rec0, const float4 *_
         }
         cp_async_commit();  // one group per batch, empty or not, so that wait_group<1> always means "batch b landed"
     };
+    // (LAZY: a coherent load -- entries the CTA sorted itself must not come through the non-coherent path)
     auto load_id = [&](uint32_t b) -> uint32_t {
         const uint32_t e = b * CF_BATCH + tid;
-        return e < total ? point_list[range.x + e] : 0u;
+        return e < total ? (LAZY ? __ldca(point_list + lbase + e) : point_list[lbase + e]) : 0u;
     };
 
     float T = 1.0f, C0 = 0.f, C1 = 0.f, C2 = 0.f, Dz = 0.f;
     uint32_t last = 0;
     bool done = !inside;
     bool warp_done = false;
+    // LAZY: per warp, the 1-based list position of the last entry of the 32-entry chunk in which its last pixel saturated
+    // (0: not yet).  Recorded where the warp leaves the list: anything inside the survivor loop costs it the uniform
+    // datapath.
+    __shared__ uint32_t s_wreach[LAZY ? CF_THREADS / 32 : 1];
+    if (LAZY && lane == 0) s_wreach[warp] = 0;
 
+    // composites the list set up in (lbase, total).  LAZY: inlined twice -- the tile's sorted prefix first, in the code
+    // of the plain kernel (its survivor loop keeps the uniform datapath, which a single copy inside the stratum loop
+    // below loses: 6 % on C2), then every stratum sorted here
+    auto composite_list = [&]() {
+    const uint32_t nbatches = (total + CF_BATCH - 1) / CF_BATCH;
     gather(0, load_id(0));
     uint32_t id_next = load_id(1);  // index for the batch after the one in flight: its latency hides behind a whole batch
     for (uint32_t b = 0; b < nbatches; b++) {
@@ -132,11 +205,38 @@ k_composite_fwd(const DevCfg c, const float4 *__restrict__ rec0, const float4 *_
             }
             if (__all_sync(0xffffffffu, done)) {
                 warp_done = true;
+                if (LAZY && lane == 0) s_wreach[warp] = pos0 + chunk + 31u + (lbase - range.x);
                 break;
             }
         }
     }
-    cp_async_wait<0>();  // nothing of ours may still be in flight into shared memory when the CTA retires
+    cp_async_wait<0>();  // nothing of ours may still be in flight into shared memory when the CTA retires (or sorts)
+    };
+    composite_list();
+    if (LAZY) {
+        uint32_t sorted = total;
+        for (;;) {
+            const bool all_done = __syncthreads_and(done);
+            const uint32_t more = all_done ? 0u
+                                           : lazy_sort_next(lazy, vt, sorted, reinterpret_cast<uint64_t *>(&stage[0]),
+                                                            const_cast<uint32_t *>(point_list) + range.x);
+            if (more == 0) {
+                if (tid == 0) {
+                    uint32_t reach = 0;
+                    for (int w = 0; w < CF_THREADS / 32; w++) reach = max(reach, s_wreach[w]);
+                    lazy_record(lazy, vt, min(reach, sorted), all_done, ranges + vt, sorted);
+                }
+                break;
+            }
+            const uint32_t prev = last;  // positions in the stratum's list count from its first entry
+            last = 0;
+            lbase = range.x + sorted;
+            total = more;
+            composite_list();
+            last = last ? last + sorted : prev;
+            sorted += more;
+        }
+    }
 
     if (inside) {
         const size_t hw = (size_t)c.H * c.W;
@@ -198,7 +298,7 @@ k_composite_fwd_ws(const DevCfg c, const float4 *__restrict__ rec0, const float4
                    const float4 *__restrict__ rec2, const uint32_t *__restrict__ point_list,
                    const uint2 *__restrict__ ranges, float *__restrict__ color, float *__restrict__ depth,
                    float *__restrict__ final_T, uint32_t *__restrict__ n_contrib, uint32_t *__restrict__ sched,
-                const uint32_t total_tiles, float *__restrict__ alpha_out) {
+                const uint32_t total_tiles, float *__restrict__ alpha_out) {  // (lists sorted whole: no lazy strata)
     __shared__ __align__(16) CpSmem sm;
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     if (tid == 0) {
@@ -354,9 +454,10 @@ k_composite_fwd_ws(const DevCfg c, const float4 *__restrict__ rec0, const float4
 }  // namespace
 
 int launch_composite_fwd(const DevCfg &c, const GsSaved &s, float *color, float *depth, cudaStream_t st, int variant,
-                         float *alpha) {
+                         float *alpha, const LazyStrata &lazy) {
     if (c.V == 0 || c.ntiles == 0) return GS_OK;
     if (variant == 2) {
+        if (lazy.cursor) return gs_set_error(GS_ERR_INVALID, "lazy strata with the warp-specialised compositor");
         // warp-specialised variant: persistent grid of SMs x resident CTAs; tiles handed out through s.sched
         constexpr int MINB_WS = 5;
         static int ctas_per_device[64] = {};   // per device: SM count x occupancy of the kernel
@@ -393,15 +494,18 @@ int launch_composite_fwd(const DevCfg &c, const GsSaved &s, float *color, float 
     constexpr int MINB = 6;
     auto launch = [&](auto kern) {
         kern<<<grid, CF_THREADS, 0, st>>>(c, s.rec0, s.rec1, s.rec2, s.point_list, s.ranges, color, depth, s.final_T, s.n_contrib,
-                                          alpha);
+                                          alpha, lazy);
     };
-    if (alpha) {
-        if (!(c.flags & GS_FLAG_DEPTH)) launch(k_composite_fwd<0, MINB, true>);
-        else if (s.depth_mode == GS_DEPTH_Z) launch(k_composite_fwd<1, MINB, true>);
-        else launch(k_composite_fwd<2, MINB, true>);
-    } else if (!(c.flags & GS_FLAG_DEPTH)) launch(k_composite_fwd<0, MINB>);
-    else if (s.depth_mode == GS_DEPTH_Z) launch(k_composite_fwd<1, MINB>);
-    else launch(k_composite_fwd<2, MINB>);
+    auto by_depth = [&](auto alpha_tag, auto lazy_tag) {
+        constexpr bool A = decltype(alpha_tag)::value, L = decltype(lazy_tag)::value;
+        if (!(c.flags & GS_FLAG_DEPTH)) launch(k_composite_fwd<0, MINB, A, L>);
+        else if (s.depth_mode == GS_DEPTH_Z) launch(k_composite_fwd<1, MINB, A, L>);
+        else launch(k_composite_fwd<2, MINB, A, L>);
+    };
+    using T_ = std::true_type;
+    using F_ = std::false_type;
+    if (alpha) lazy.cursor ? by_depth(T_{}, T_{}) : by_depth(T_{}, F_{});
+    else lazy.cursor ? by_depth(F_{}, T_{}) : by_depth(F_{}, F_{});
     GS_CUDA_OK(cudaGetLastError());
     return GS_OK;
 }

@@ -157,6 +157,10 @@ class OracleRender:
         self.num_pairs = int(self.lib.gso_num_pairs(self.handle))
         self.has_sh = shs is not None
         self.has_scales = scales is not None
+        # what the SH colour was evaluated from: lets a test recompute the value the clamp at 0 saw
+        self.means3D, self.shs = means3D, shs
+        self.campos = np.asarray(s.campos, np.float64).reshape(3)
+        self.sh_eval_degree = min(int(s.sh_degree), int(s.sh_eval_max_degree))
 
     def _view(self, fn, dtype, shape):
         p = getattr(self.lib, fn)(self.handle)
@@ -190,6 +194,8 @@ class OracleRender:
     def px_fragile(self): return self._view("gso_px_fragile", np.uint8, (self.H, self.W)).astype(bool)
     @property
     def geom_fragile(self): return self._view("gso_geom_fragile", np.uint8, (self.P,)).astype(bool)
+    @property
+    def geom_fragile_bits(self): return self._view("gso_geom_fragile", np.uint8, (self.P,))   # 1 radius, 2 cull, 4 rect
     @property
     def clamped(self): return self._view("gso_clamped", np.uint8, (self.P, 3)).astype(bool)
 

@@ -87,7 +87,7 @@ class DepthModeOracle:
     def backward(self, dL_dcolor, w) -> dict:
         g = self.ob_color.backward(dL_dcolor)
         gd = self.ob_depth.backward(np.repeat(np.asarray(w, np.float64)[:, None] / 3.0, 3, axis=1))
-        for k in ("means3D", "opacities", "scales", "rotations", "cov3D_precomp"):
+        for k in ("means3D", "means2D", "opacities", "scales", "rotations", "cov3D_precomp"):
             if g[k] is not None:
                 g[k] = g[k] + gd[k]
         # dL/dz_s per (view, Gaussian): the fake colour's gradient through f'(z) dz/dz_s

@@ -256,9 +256,9 @@ GS_API int gs_backward_ex(GsContext *ctx, const GsConfig *cfg, const GsInputs *i
  * GS_DEPTH_LOG's clamp gives zero), the accumulated opacity and the anti-aliasing factor.  A guard-band-clamped t.x / t.y
  * has no gradient, an invisible or culled (view, Gaussian) pair contributes nothing, and the 0.99 alpha clamp passes the
  * gradient straight through, as for the means.  The values are in the view-scaled scene (GsConfig.view_scale), so they
- * are gradients of the matrices as passed; tanfov, near, far, bg and the intrinsics get none.  Each pointer is device
- * memory or NULL (not wanted); the arrays are written, not accumulated.  Deterministic: per-warp partials summed in a
- * fixed order, in both modes. */
+ * are gradients of the matrices as passed.  tanfov gets its gradient from gs_backward_cam_tanfov; near, far and bg get
+ * none.  Each pointer is device memory or NULL (not wanted); the arrays are written, not accumulated.  Deterministic:
+ * per-warp partials summed in a fixed order, in both modes. */
 typedef struct GsCameraGrads {
     float *dL_dviewmatrix;  /* device [V,16]: the flat transposed world-to-camera matrix (GsConfig.viewmatrix) */
     float *dL_dprojmatrix;  /* device [V,16]: the flat transposed full projection (GsConfig.projmatrix) */
@@ -271,6 +271,18 @@ typedef struct GsCameraGrads {
 GS_API int gs_backward_cam(GsContext *ctx, const GsConfig *cfg, const GsInputs *in, const GsSaved *saved,
                            const GsOutGrads *gout, const GsAlpha *alpha, const GsInGrads *gin, const GsCameraGrads *cam,
                            void *stream);
+
+/* gs_backward_cam that also writes dL/dtanfov (device [V,2], x then y per view; NULL = not wanted): the partial derivative
+ * of what the kernels compute with respect to the tangent of the half field of view (GsConfig.tanfov, or tanfovx/tanfovy
+ * for every view) as passed, projmatrix held fixed -- its 1/tanfov entries are a separate input, with their own gradient
+ * in cam.  tanfov enters through the focal lengths of the projection Jacobian, fx = W / (2 tanfovx), and through the
+ * guard-band clamp of the Jacobian's evaluation point, t.x = clamp(t.x / t.z, +-guard_band tanfovx) t.z (y likewise).
+ * It reaches every output that reads the 2-D covariance: colour, the depth channel, the accumulated opacity and the
+ * anti-aliasing factor.  Culling, radii and tile binning are discrete and give none.  The camera outputs in cam are the
+ * bytes gs_backward_cam writes, with or without dL_dtanfov.  Same refusals as gs_backward_cam. */
+GS_API int gs_backward_cam_tanfov(GsContext *ctx, const GsConfig *cfg, const GsInputs *in, const GsSaved *saved,
+                                  const GsOutGrads *gout, const GsAlpha *alpha, const GsInGrads *gin,
+                                  const GsCameraGrads *cam, float *dL_dtanfov, void *stream);
 
 GS_API void gs_saved_free(GsContext *ctx, GsSaved *saved, void *stream);
 

@@ -173,6 +173,9 @@ SYMBOLS = {
                                POINTER(GsAlpha), POINTER(GsInGrads), c_void_p]),
     "gs_backward_cam": (c_int, [c_void_p, POINTER(GsConfig), POINTER(GsInputs), c_void_p, POINTER(GsOutGrads),
                                 POINTER(GsAlpha), POINTER(GsInGrads), POINTER(GsCameraGrads), c_void_p]),
+    "gs_backward_cam_tanfov": (c_int, [c_void_p, POINTER(GsConfig), POINTER(GsInputs), c_void_p, POINTER(GsOutGrads),
+                                       POINTER(GsAlpha), POINTER(GsInGrads), POINTER(GsCameraGrads), c_void_p,
+                                       c_void_p]),
     "gs_render_host_ex": (c_int, [c_void_p, POINTER(GsConfig), POINTER(GsInputs), POINTER(GsOutputs), POINTER(GsAlpha),
                                   c_void_p]),
     "gs_set_profiling": (c_int, [c_void_p, c_int]),

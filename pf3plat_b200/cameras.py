@@ -69,10 +69,12 @@ def make_view_batch(extrinsics, intrinsics, near, far, scale_invariant: bool = T
     render_depth_cuda's camera gradient (cuda_splatting.py:239-242).  `projmatrix`, `campos` and `tanfov` stay
     detached, and `near` / `far` get no gradient.
 
-    camera_gradients (None = rasterizer.get_camera_gradients()): on, the three camera inputs follow render_cuda's own
-    torch glue instead -- the translation of the extrinsics rescaled by 1/near, then inverted; projmatrix = view @ P with
-    P detached; campos = the rescaled translation -- so that the full camera gradient reaches the extrinsics in all 16
-    entries as that glue would carry it."""
+    camera_gradients (None = rasterizer.get_camera_gradients()): on, with extrinsics or intrinsics that require grad, the
+    camera inputs follow render_cuda's own torch glue instead -- the translation of the extrinsics rescaled by 1/near,
+    then inverted; projmatrix = view @ P, P from the fov of the intrinsics (get_fov, all nine entries); campos = the
+    rescaled translation; tanfov = tan(fov / 2) -- so that the full camera gradient reaches the extrinsics in all 16
+    entries and the intrinsics in all 9, as that glue would carry it.  Off, the intrinsics get no gradient.  The CPU path
+    is that glue in plain tensor code, differentiable throughout."""
     if extrinsics.is_cuda:
         return _make_view_batch_cuda(extrinsics, intrinsics, near, far, scale_invariant, camera_gradients)
     if scale_invariant:
@@ -114,7 +116,8 @@ def _make_view_batch_cuda(extrinsics, intrinsics, near, far, scale_invariant: bo
     if camera_gradients is None:
         from .rasterizer import get_camera_gradients
         camera_gradients = get_camera_gradients()
-    if camera_gradients and extrinsics.requires_grad and torch.is_grad_enabled():
+    intr_grad = intrinsics.requires_grad
+    if camera_gradients and (extrinsics.requires_grad or intr_grad) and torch.is_grad_enabled():
         # The kernel's values (plus exact zeros) with the gradients of render_cuda's glue (cuda_splatting.py:64-86)
         e = extrinsics.clone()
         inv_near = (1.0 / near.detach().to(dev, e.dtype))
@@ -123,13 +126,17 @@ def _make_view_batch_cuda(extrinsics, intrinsics, near, far, scale_invariant: bo
         vt = torch.linalg.inv(e).transpose(-1, -2)
         with torch.no_grad():
             nr_s, fr_s = (nr * scale, fr * scale) if scale_invariant else (nr, fr)
-            fov_x, fov_y = get_fov(intr).unbind(-1)
-            pt = get_projection_matrix(nr_s, fr_s, fov_x, fov_y).transpose(-1, -2).to(vt.dtype)
+        # the intrinsics as given when they require grad, else the kernel's fp32 copy (no graph: P is a constant)
+        fov_x, fov_y = get_fov(intrinsics.to(dev) if intr_grad else intr).unbind(-1)
+        pt = get_projection_matrix(nr_s.to(fov_x.dtype), fr_s.to(fov_x.dtype), fov_x, fov_y).transpose(-1, -2).to(vt.dtype)
         full = vt @ pt
         cp = e[:, :3, 3]
         view = view + (vt - vt.detach()).to(view.dtype)
         proj = proj + (full - full.detach()).to(proj.dtype)
         campos = campos + (cp - cp.detach()).to(campos.dtype)
+        if intr_grad:
+            tan = torch.stack(((0.5 * fov_x).tan(), (0.5 * fov_y).tan()), dim=-1)
+            tanfov = tanfov + (tan - tan.detach()).to(tanfov.dtype)
     elif extrinsics.requires_grad and torch.is_grad_enabled():
         # The kernel's values (plus exact zeros) with the gradient of a torch expression of the view matrix.  The
         # expression rescales the translation of extrinsics^-1 rather than that of the extrinsics

@@ -658,7 +658,8 @@ extern "C" int gs_forward_ex(GsContext *ctx, const GsConfig *cfg, const GsInputs
 
 namespace {
 int backward(GsContext *ctx, const GsConfig *cfg, const GsInputs *in, const GsSaved *saved, const GsOutGrads *gout,
-             const float *dL_dalpha, const GsInGrads *gin, void *stream, const GsCameraGrads *cam = nullptr) {
+             const float *dL_dalpha, const GsInGrads *gin, void *stream, const GsCameraGrads *cam = nullptr,
+             float *dL_dtanfov = nullptr) {
     if (!ctx || !saved || !gout || !gin) return gs_set_error(GS_ERR_INVALID, "null argument");
     int rc = validate(cfg, in);
     if (rc != GS_OK) return rc;
@@ -704,6 +705,7 @@ int backward(GsContext *ctx, const GsConfig *cfg, const GsInputs *in, const GsSa
         if (cam && cam->dL_dviewmatrix) GS_CUDA_OK(cudaMemsetAsync(cam->dL_dviewmatrix, 0, (size_t)c.V * 16 * 4, st));
         if (cam && cam->dL_dprojmatrix) GS_CUDA_OK(cudaMemsetAsync(cam->dL_dprojmatrix, 0, (size_t)c.V * 16 * 4, st));
         if (cam && cam->dL_dcampos) GS_CUDA_OK(cudaMemsetAsync(cam->dL_dcampos, 0, (size_t)c.V * 3 * 4, st));
+        if (cam && dL_dtanfov) GS_CUDA_OK(cudaMemsetAsync(dL_dtanfov, 0, (size_t)c.V * 2 * 4, st));
         return GS_OK;
     }
 
@@ -734,7 +736,8 @@ int backward(GsContext *ctx, const GsConfig *cfg, const GsInputs *in, const GsSa
     }
     {
         StageTimer t(ctx, GS_STAGE_PREPROCESS_BWD, st);
-        rc = launch_preprocess_bwd(c, di, *saved, acc, g, st, (cfg->tuning & GS_TUNE_PBWD_2PHASE) ? 1 : 0, da, dm, cam);
+        rc = launch_preprocess_bwd(c, di, *saved, acc, g, st, (cfg->tuning & GS_TUNE_PBWD_2PHASE) ? 1 : 0, da, dm, cam,
+                                   dL_dtanfov);
         if (rc != GS_OK) return rc;
     }
     ctx->stats.kernel_launches += 2;  // k_composite_bwd, k_preprocess_bwd
@@ -760,6 +763,13 @@ extern "C" int gs_backward_cam(GsContext *ctx, const GsConfig *cfg, const GsInpu
                                void *stream) {
     if (!cam) return gs_set_error(GS_ERR_INVALID, "null camera-gradient request");
     return backward(ctx, cfg, in, saved, gout, alpha ? alpha->dL_dalpha : nullptr, gin, stream, cam);
+}
+
+extern "C" int gs_backward_cam_tanfov(GsContext *ctx, const GsConfig *cfg, const GsInputs *in, const GsSaved *saved,
+                                      const GsOutGrads *gout, const GsAlpha *alpha, const GsInGrads *gin,
+                                      const GsCameraGrads *cam, float *dL_dtanfov, void *stream) {
+    if (!cam) return gs_set_error(GS_ERR_INVALID, "null camera-gradient request");
+    return backward(ctx, cfg, in, saved, gout, alpha ? alpha->dL_dalpha : nullptr, gin, stream, cam, dL_dtanfov);
 }
 
 extern "C" int gs_mark_visible(GsContext *ctx, const GsConfig *cfg, const float *means3D, uint8_t *present,

@@ -158,7 +158,8 @@ int launch_composite_bwd(const DevCfg &c, const GsSaved &s, const float *dL_dcol
 int launch_preprocess_bwd(const DevCfg &c, const DevInputs &in, const GsSaved &s, const float *grad_acc,
                           const GsInGrads &g, cudaStream_t st, int variant = 0 /* 1: the two-phase kernel (GS_TUNE_PBWD_2PHASE) */,
                           const DetAcc &det = DetAcc{}, const DepthMode &dm = DepthMode{},
-                          const GsCameraGrads *cam = nullptr /* non-NULL: also the camera gradient */);
+                          const GsCameraGrads *cam = nullptr /* non-NULL: also the camera gradient */,
+                          float *dL_dtanfov = nullptr /* with cam: also dL/dtanfov [V,2] */);
 // bytes of DetAcc::view_z for a configuration
 size_t det_view_z_bytes(const DevCfg &c);
 // bytes of DetAcc::view_z the camera gradient needs, in both modes: per-warp slots of 32 floats per view

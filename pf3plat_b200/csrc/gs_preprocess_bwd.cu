@@ -191,10 +191,10 @@ __device__ __forceinline__ void view_z_grad(const GsInGrads &g, const DetAcc &de
     }
 }
 
-// Camera gradient (GsCameraGrads): 27 terms per (view, Gaussian) pair in the slots of det.view_z, [V][warps][GS_CAM_NC]:
+// Camera gradient (GsCameraGrads): 29 terms per (view, Gaussian) pair in the slots of det.view_z, [V][warps][GS_CAM_NC]:
 //   0..11  dL/dviewmatrix[4k + r] at component 3k + r (k = 0..3, r = 0..2; the fourth column is never read)
 //   12..23 dL/dprojmatrix[4k + c] at component 12 + 3k + i, c = (0, 1, 3)[i] (the third column feeds no output)
-//   24..26 dL/dcampos, 27..31 zero (one component per lane of k_camera_finalize)
+//   24..26 dL/dcampos, 27..28 dL/dtanfov (x, y), 29..31 zero (one component per lane of k_camera_finalize)
 // Each of the three groups is reduced where it is computed, which keeps few of the terms live at once.
 constexpr int GS_CAM_NC = 32;
 
@@ -240,7 +240,7 @@ __device__ __forceinline__ const float *load_det_acc(const DetAcc &det, size_t o
 // joins dL/d(a, b, c) ahead of the cov2D -> cov3D and cov2D -> J -> mean chains (DESIGN.md 5.5).  The AA = false kernels
 // are the ones without it, instruction for instruction.
 // CAM: also the camera gradient (GsCameraGrads), into the slots of det.view_z (GS_CAM_NC components, in both modes), which
-// k_camera_finalize turns into dL/dviewmatrix, dL/dprojmatrix and dL/dcampos (DESIGN.md 5.5).  Never
+// k_camera_finalize turns into dL/dviewmatrix, dL/dprojmatrix, dL/dcampos and dL/dtanfov (DESIGN.md 5.5).  Never
 // with VIEW_Z = 1: the full gradient contains the z column.  The CAM = false kernels are the ones without it.
 template <bool HAS_SH, int MINB, int VIEW_Z = 0, bool DET = false, bool B4 = false, bool AA = false, bool CAM = false>
 __global__ void __launch_bounds__(PB_THREADS, MINB)
@@ -344,6 +344,8 @@ k_preprocess_bwd(const DevCfg c, const DevInputs in, const uint8_t *__restrict__
             const float3 m = make_float3(mean.x * s, mean.y * s, mean.z * s);
             const float cv[6] = {c6[0] * s2, c6[1] * s2, c6[2] * s2, c6[3] * s2, c6[4] * s2, c6[5] * s2};
             float gm[3] = {0.f, 0.f, 0.f};  // dL/dm (view-scaled mean)
+            // CAM: components 24..31 of the slot: dL/dcampos = -dL/dd (d = m - campos), then dL/dtanfov
+            float gcp[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
             // ---- conic -> cov2D -> cov3D, mean (through J) ----
             {
                 ProjJac j;
@@ -424,6 +426,11 @@ k_preprocess_bwd(const DevCfg c, const DevInputs in, const uint8_t *__restrict__
                     }
                     cv[9] = dt[0]; cv[10] = dt[1]; cv[11] = dt[2];
                     view_partial<GS_CAM_NC>(det.view_z, v, 0, cv);
+                    // fx = W / (2 tanfovx) scales J00 and J02, so dL/dtanfovx = -(dL/dJ00 J00 + dL/dJ02 J02) / tanfovx;
+                    // a clamped t.x = +-guard_band tanfovx t.z makes J02 independent of tanfovx and drops its term
+                    // (y likewise)
+                    gcp[3] = -(dJ00 * J00 + (j.xin ? dJ02 * J02 : 0.0f)) / cam.tanfovx;
+                    gcp[4] = -(dJ11 * J11 + (j.yin ? dJ12 * J12 : 0.0f)) / cam.tanfovy;
                 }
             }
             // ---- mean2D (NDC units) -> mean through the perspective divide ----
@@ -454,7 +461,6 @@ k_preprocess_bwd(const DevCfg c, const DevInputs in, const uint8_t *__restrict__
             gm[1] += cam.view[6] * gz;
             gm[2] += cam.view[10] * gz;
             if (VIEW_Z == 1 || (VIEW_Z == 2 && g.dL_dviewmatrix_z)) view_z_grad<DET>(g, det, v, gz * m.x, gz * m.y, gz * m.z, gz);
-            float gcp[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};   // CAM: dL/dcampos = -dL/dd, d = m - campos
             // ---- colour -> SH coefficients and mean (view direction) ----
             if (HAS_SH) {
                 const float d[3] = {m.x - cam.campos[0], m.y - cam.campos[1], m.z - cam.campos[2]};
@@ -936,8 +942,9 @@ __global__ void k_view_z_finalize(int V, int warps, const float *__restrict__ vi
 // its own layouts (zeros where an entry feeds nothing; a NULL output is skipped).  Fixed order, so deterministic: lane x
 // of row y adds component x of the slots w = y, y + 32, y + 64, ... in turn (each row reads whole 128-byte slots), then
 // row 0 adds the 32 row sums in row order.  One CTA of 32 x 32 threads per view: a view's slots are spread over 32
-// sequential chains instead of one (a scene of 500k Gaussians has 15 625 slots per view).
-__global__ void __launch_bounds__(1024) k_camera_finalize(int warps, const float *__restrict__ slots, GsCameraGrads out) {
+// sequential chains instead of one (a scene of 500k Gaussians has 15 625 slots per view).  dL_dtanfov: [V,2] or NULL.
+__global__ void __launch_bounds__(1024) k_camera_finalize(int warps, const float *__restrict__ slots, GsCameraGrads out,
+                                                          float *__restrict__ dL_dtanfov) {
     __shared__ float part[32][33];
     const int v = blockIdx.x, k = threadIdx.x, r = threadIdx.y;
     const float *p = slots + (size_t)v * warps * GS_CAM_NC + k;
@@ -955,6 +962,8 @@ __global__ void __launch_bounds__(1024) k_camera_finalize(int warps, const float
             if (out.dL_dprojmatrix) out.dL_dprojmatrix[v * 16 + 4 * i + (j == 2 ? 3 : j)] = t;
         } else if (k < 27) {
             if (out.dL_dcampos) out.dL_dcampos[v * 3 + k - 24] = t;
+        } else if (k < 29) {
+            if (dL_dtanfov) dL_dtanfov[v * 2 + k - 27] = t;
         }
     } else if (r == 1 && k < 8) {   // the entries that feed nothing: the view matrix's 4th column, Pf's 3rd
         if (k < 4 && out.dL_dviewmatrix) out.dL_dviewmatrix[v * 16 + 4 * k + 3] = 0.f;
@@ -1000,15 +1009,15 @@ size_t camera_grad_scratch_bytes(const DevCfg &c) { return (size_t)view_z_warps(
 // g.dL_dviewmatrix_z non-NULL selects the VIEW_Z kernels; the caller has zeroed it (the kernels accumulate into it, or in
 // deterministic mode k_view_z_finalize writes it).  det.acc non-NULL selects the deterministic kernels.  cam non-NULL
 // selects the camera-gradient kernels (never with dL_dviewmatrix_z): det.view_z then holds camera_grad_scratch_bytes of
-// per-warp slots, in both modes.
+// per-warp slots, in both modes, and dL_dtanfov (may be NULL) receives the tanfov gradient.
 int launch_preprocess_bwd(const DevCfg &c, const DevInputs &in, const GsSaved &s, const float *grad_acc,
                           const GsInGrads &g, cudaStream_t st, int variant, const DetAcc &det, const DepthMode &dm,
-                          const GsCameraGrads *cam) {
+                          const GsCameraGrads *cam, float *dL_dtanfov) {
     if (c.P == 0) return GS_OK;
     if (cam) {
         const int rc = launch_preprocess_bwd_cam<true>(c, in, s, grad_acc, g, st, variant, det, dm);
         if (rc != GS_OK) return rc;
-        k_camera_finalize<<<c.V, dim3(32, 32), 0, st>>>(view_z_warps(c), det.view_z, *cam);
+        k_camera_finalize<<<c.V, dim3(32, 32), 0, st>>>(view_z_warps(c), det.view_z, *cam, dL_dtanfov);
         GS_CUDA_OK(cudaGetLastError());
         return GS_OK;
     }

@@ -168,9 +168,9 @@ class BatchSettings(NamedTuple):
     # highest SH degree evaluated (GsConfig.sh_eval_max_degree): 3, or 4 to evaluate and train band 4 of a 25-coefficient
     # block; None = the process-wide setting (set_sh_eval_max_degree)
     sh_eval_max_degree: Optional[int] = None
-    # also differentiate the cameras: a viewmatrix, projmatrix or campos that requires grad gets the full gradient of every
-    # output (gs_backward_cam) instead of the depth channel's z column alone; None = the process-wide setting
-    # (set_camera_gradients, default off)
+    # also differentiate the cameras: a viewmatrix, projmatrix, campos or tanfov that requires grad gets the full gradient
+    # of every output (gs_backward_cam_tanfov) instead of the depth channel's z column alone; None = the process-wide
+    # setting (set_camera_gradients, default off)
     camera_gradients: Optional[bool] = None
     # what the depth channel (with_depth) composites: PF3plat's DepthRenderingMode -- "depth" (camera-space z of the
     # view-scaled scene), "disparity", "relative_disparity" or "log" (f(z) of render_depth_cuda at the unscaled z)
@@ -260,9 +260,9 @@ _camera_gradients = False
 def set_camera_gradients(enabled: bool) -> None:
     """Process-wide camera-gradient setting used when BatchSettings.camera_gradients (or the `camera_gradients` argument of
     the drop-in, render_views, decoder_forward) is None: False (the default: as in the reference op, only the depth
-    channel reaches the view matrix's z column) or True (viewmatrix, projmatrix and campos get the gradient of colour,
-    depth, alpha and the anti-aliasing factor; make_view_batch carries it on to the extrinsics).  A forward's backward
-    uses the setting of that forward."""
+    channel reaches the view matrix's z column) or True (viewmatrix, projmatrix, campos and a tanfov tensor get the
+    gradient of colour, depth, alpha and the anti-aliasing factor; make_view_batch carries it on to the extrinsics and
+    the intrinsics).  A forward's backward uses the setting of that forward."""
     global _camera_gradients
     _camera_gradients = bool(enabled)
 
@@ -305,18 +305,19 @@ def _make_config(bs: BatchSettings, S: int, P: int, M: int, keep: list) -> GsCon
 class _RasterizeBatch(torch.autograd.Function):
     """The reference's _RasterizeGaussians (SURVEY.md section 3.4), batched over views.
 
-    `viewmatrix`, `projmatrix` and `campos` are bs.viewmatrix, bs.projmatrix and bs.campos, handed in as tensor inputs so
-    that autograd can route gradients to them.  By default the view matrix gets one only through the fused depth channel
+    `viewmatrix`, `projmatrix`, `campos` and `tanfov` are bs.viewmatrix, bs.projmatrix, bs.campos and bs.tanfov, handed
+    in as tensor inputs so that autograd can route gradients to them.  By default the view matrix gets one only through the fused depth channel
     (bs.with_depth), as the reference's depth pass gives its cameras one through its fake colour z
     (cuda_splatting.py:239-242): dL/dviewmatrix is zero outside the z column, and None when the depth is not part of the
-    loss; projmatrix and campos get None.  Colour, projection and culling give the cameras no gradient, as in the
-    reference op.  With bs.camera_gradients, the three get the full gradient of every output the loss reads
-    (gs_backward_cam), the depth channel's included.  bs.with_alpha appends the accumulated opacity (gs_forward_ex /
+    loss; projmatrix, campos and tanfov get None.  Colour, projection and culling give the cameras no gradient, as in the
+    reference op.  With bs.camera_gradients, the four get the full gradient of every output the loss reads
+    (gs_backward_cam_tanfov), the depth channel's included; tanfov's is the partial derivative with projmatrix held
+    fixed.  bs.with_alpha appends the accumulated opacity (gs_forward_ex /
     gs_backward_ex).  Under torch.use_deterministic_algorithms(True) the backward is bit-reproducible."""
 
     @staticmethod
     def forward(ctx, means3D, means2D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp, viewmatrix,
-                projmatrix, campos, bs: BatchSettings):
+                projmatrix, campos, tanfov, bs: BatchSettings):
         # an output the loss does not use arrives in backward as None instead of a zero tensor: a colour-only loss
         # then gives the view matrices no gradient at all (and the kernels read no depth gradient: the same sums)
         ctx.set_materialize_grads(False)
@@ -345,7 +346,7 @@ class _RasterizeBatch(torch.autograd.Function):
             depth = torch.empty((V, H, W), dtype=torch.float32, device=dev) if bs.with_depth else None
             gout = GsOutputs(_ptr(color), _ptr(radii), _ptr(depth))
             alpha = torch.empty((V, H, W), dtype=torch.float32, device=dev) if bs.with_alpha else None
-            cam_leaves = (viewmatrix, projmatrix, campos)
+            cam_leaves = (viewmatrix, projmatrix, campos, tanfov)
             want_cam = bool(bs.camera_gradients) and any(t is not None and t.requires_grad for t in cam_leaves)
             want_view_z = bs.with_depth and viewmatrix.requires_grad and not want_cam
             needs_grad = want_cam or want_view_z or any(t is not None and t.requires_grad for t in
@@ -375,7 +376,8 @@ class _RasterizeBatch(torch.autograd.Function):
             ctx.dims = (S, P, V, M, H, W)
             ctx.want_means2D = means2D is not None and means2D.requires_grad
             ctx.view_z = (viewmatrix.shape, viewmatrix.dtype) if want_view_z else None
-            ctx.cam = [(t.shape, t.dtype, t.device, t.requires_grad) for t in cam_leaves] if want_cam else None
+            ctx.cam = [(None, None, None, False) if t is None else (t.shape, t.dtype, t.device, t.requires_grad)
+                       for t in cam_leaves] if want_cam else None
         ctx.mark_non_differentiable(radii)
         return (color, radii) + ((depth,) if bs.with_depth else ()) + ((alpha,) if bs.with_alpha else ())
 
@@ -416,14 +418,15 @@ class _RasterizeBatch(torch.autograd.Function):
                 "dL_dviewmatrix_z": e(V, 4) if ctx.view_z is not None and gdep is not None else None,
             }
             ig = GsInGrads(**{k: _ptr(t) for k, t in g.items()})
-            gcam = [e(V, 16), e(V, 16), e(V, 3)] if ctx.cam is not None else None
+            # (dL/dtanfov only when tanfov requires grad: the other three are the same bytes with or without it)
+            gcam = [e(V, 16), e(V, 16), e(V, 3), e(V, 2) if ctx.cam[3][3] else None] if ctx.cam is not None else None
             with _context_lock(dev, stream_ptr):
                 if gcam is not None:
                     galpha = _f32c(grad_alpha)
-                    rc = _capi.lib().gs_backward_cam(
+                    rc = _capi.lib().gs_backward_cam_tanfov(
                         gctx, ctypes.byref(cfg), ctypes.byref(gin), ctx.handle.ptr, ctypes.byref(og),
                         ctypes.byref(_capi.GsAlpha(None, _ptr(galpha))), ctypes.byref(ig),
-                        ctypes.byref(_capi.GsCameraGrads(*[_ptr(t) for t in gcam])), stream_ptr)
+                        ctypes.byref(_capi.GsCameraGrads(*[_ptr(t) for t in gcam[:3]])), _ptr(gcam[3]), stream_ptr)
                 elif grad_alpha is not None:
                     galpha = _f32c(grad_alpha)
                     rc = _capi.lib().gs_backward_ex(gctx, ctypes.byref(cfg), ctypes.byref(gin), ctx.handle.ptr,
@@ -433,10 +436,10 @@ class _RasterizeBatch(torch.autograd.Function):
                     rc = _capi.lib().gs_backward(gctx, ctypes.byref(cfg), ctypes.byref(gin), ctx.handle.ptr,
                                                  ctypes.byref(og), ctypes.byref(ig), stream_ptr)
                 _capi.check(rc)
-            gview = gproj = gcampos = None
+            gview = gproj = gcampos = gtan = None
             if gcam is not None:
-                gview, gproj, gcampos = (gt.reshape(shape).to(device, dtype) if req else None
-                                         for gt, (shape, dtype, device, req) in zip(gcam, ctx.cam))
+                gview, gproj, gcampos, gtan = (gt.reshape(shape).to(device, dtype) if req else None
+                                               for gt, (shape, dtype, device, req) in zip(gcam, ctx.cam))
             if g["dL_dviewmatrix_z"] is not None:
                 # flat entries 2, 6, 10, 14 of the transposed matrix: its z column
                 gview = torch.zeros((V, 4, 4), dtype=torch.float32, device=dev)
@@ -444,7 +447,7 @@ class _RasterizeBatch(torch.autograd.Function):
                 shape, dtype = ctx.view_z
                 gview = gview.reshape(shape).to(dtype)
         return (g["dL_dmeans3D"], g["dL_dmeans2D"], g["dL_dshs"], g["dL_dcolors"], g["dL_dopacities"],
-                g["dL_dscales"], g["dL_drotations"], g["dL_dcov3D"], gview, gproj, gcampos, None)
+                g["dL_dscales"], g["dL_drotations"], g["dL_dcov3D"], gview, gproj, gcampos, gtan, None)
 
 
 def rasterize_batch(bs: BatchSettings, means3D, opacities, shs=None, colors_precomp=None, scales=None,
@@ -453,13 +456,13 @@ def rasterize_batch(bs: BatchSettings, means3D, opacities, shs=None, colors_prec
     (V,P,3); scales (S,P,3); rotations (S,P,4); cov3D_precomp (S,P,6); means2D (V,P,3) (gradient sink only).
     Returns (color (V,3,H,W), radii (V,P)[, depth (V,H,W)][, alpha (V,H,W)]).  With bs.with_depth, a bs.viewmatrix that
     requires grad gets dL/ddepth's gradient in its z column (see _RasterizeBatch); bs.with_alpha appends the accumulated
-    opacity 1 - T_final.  With bs.camera_gradients, bs.viewmatrix, bs.projmatrix and bs.campos that require grad get the
-    full camera gradient instead."""
+    opacity 1 - T_final.  With bs.camera_gradients, bs.viewmatrix, bs.projmatrix, bs.campos and bs.tanfov that require
+    grad get the full camera gradient instead."""
     _check_exclusive(shs, colors_precomp, scales, rotations, cov3D_precomp)
     # means2D exists in the reference op only as a sink for the screen-space gradient (cuda_splatting.py:93-97); the
     # batched entry neither allocates nor fills it unless the caller passes one
     return _RasterizeBatch.apply(means3D, means2D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp,
-                                 bs.viewmatrix, bs.projmatrix, bs.campos, bs)
+                                 bs.viewmatrix, bs.projmatrix, bs.campos, bs.tanfov, bs)
 
 
 def _check_exclusive(shs, colors_precomp, scales, rotations, cov3D_precomp):
@@ -516,7 +519,9 @@ class GaussianRasterizer(nn.Module):
         GaussianRasterizationSettings.antialiasing, which this 12-field settings tuple does not carry); None = the
         process-wide setting (set_antialiasing).  `camera_gradients`: viewmatrix, projmatrix and campos of the settings
         get the full gradient of the outputs (None = the process-wide setting, set_camera_gradients); off, the reference
-        op's behaviour, they get none."""
+        op's behaviour, they get none.  tanfovx and tanfovy get none either way: the settings carry them as Python
+        floats (an unmodified render_cuda hands over `.item()`s), so no gradient could reach the intrinsics through them;
+        render_views / decoder_forward give the intrinsics theirs."""
         _check_exclusive(shs, colors_precomp, scales, rotations, cov3D_precomp)
         u = lambda t: None if t is None else t.unsqueeze(0)
         cam = _camera_gradients if camera_gradients is None else bool(camera_gradients)
@@ -524,5 +529,5 @@ class GaussianRasterizer(nn.Module):
             with_alpha=bool(return_alpha), antialiasing=None if antialiasing is None else bool(antialiasing),
             camera_gradients=cam)
         out = _RasterizeBatch.apply(u(means3D), u(means2D), u(shs), u(colors_precomp), u(opacities), u(scales),
-                                    u(rotations), u(cov3D_precomp), bs.viewmatrix, bs.projmatrix, bs.campos, bs)
+                                    u(rotations), u(cov3D_precomp), bs.viewmatrix, bs.projmatrix, bs.campos, None, bs)
         return tuple(o[0] for o in out)

@@ -46,9 +46,10 @@ def render_views(extrinsics, intrinsics, near, far, image_shape, background_colo
     with_alpha: also return the accumulated opacity alpha (B,h,w) = 1 - T_final, last: (color[, depth], alpha).
     antialiasing: the screen-space filter with opacity compensation (BatchSettings.antialiasing); None = the
     process-wide setting (rasterizer.set_antialiasing, default off).
-    camera_gradients: extrinsics that require grad get the full gradient of every output (colour, depth, alpha, the
-    anti-aliasing factor) through render_cuda's own camera glue (make_view_batch); None = the process-wide setting
-    (rasterizer.set_camera_gradients, default off: only the depth channel reaches them)."""
+    camera_gradients: extrinsics and intrinsics that require grad get the full gradient of every output (colour, depth,
+    alpha, the anti-aliasing factor) through render_cuda's own camera glue (make_view_batch; the intrinsics through the
+    fov, into tanfov and P); None = the process-wide setting (rasterizer.set_camera_gradients, default off: only the
+    depth channel reaches the extrinsics, and the intrinsics get none)."""
     assert use_sh or gaussian_sh_coefficients.shape[-1 if sh_layout == "g_xyz_n" else -2] == 1
     h, w = image_shape
     if camera_gradients is None:
@@ -114,7 +115,8 @@ def decoder_forward(means, covariances, harmonics, opacities, extrinsics, intrin
     antialiasing: as render_views; the opacity compensation gives the extrinsics no gradient either.
     camera_gradients (None = rasterizer.get_camera_gradients(), default off): the extrinsics get the full gradient of
     every output instead -- colour, depth (the z-column route above is then part of it, not added again), alpha and
-    the anti-aliasing factor -- for photometric pose training and test-time pose refinement."""
+    the anti-aliasing factor -- for photometric pose training and test-time pose refinement; intrinsics that require
+    grad get theirs too, in all nine entries (focal refinement, calibration-free use)."""
     b, v = extrinsics.shape[:2]
     flat = lambda t: t.reshape(b * v, *t.shape[2:])
     bg = background_color.reshape(1, 3).expand(b * v, 3)

@@ -1,10 +1,11 @@
-"""What the camera gradient (gs_backward_cam) costs.  Forward + backward with the setting off and on, alternated in one
-process, medians over rounds; besides the times, every stage of the library (gs_get_stage_ms, in a separate profiled pass)
+"""What the camera gradient (gs_backward_cam_tanfov) costs.  Forward + backward with the setting off, on for the
+extrinsics, and on for the extrinsics and the intrinsics, alternated in one process, medians over rounds; besides the times, every stage of the library (gs_get_stage_ms, in a separate profiled pass)
 and what is left of the step outside the library.  Prints one JSON line with the card's name, power limit and clock, read in the same run.
   * PF3plat's training shape: b = 14 scenes x v = 3 views, 131072 Gaussians per scene (2 x 256 x 256), 256x256,
     decoder_forward(depth_mode="depth") on poses that require grad, loss = MSE on the colour + mean depth (off: the depth
-    channel's z column reaches the poses; on: the full gradient);
-  * C2: 500k Gaussians x 8 views x 256x256, M = 25, loss = <W, colour>, the three camera inputs requiring grad.
+    channel's z column reaches the poses; on: the full gradient; with the intrinsics: they require grad too);
+  * C2: 500k Gaussians x 8 views x 256x256, M = 25, loss = <W, colour>, the three camera inputs requiring grad (and
+    tanfov, with the intrinsics).
 Usage: python scripts/bench_camera_grad.py [--steps K] [--warmup W] [--rounds R]"""
 import argparse
 import json
@@ -20,20 +21,21 @@ from pf3plat_b200.render import decoder_forward  # noqa: E402
 from pf3plat_b200.synthetic import make_pixel_aligned_scene, make_scene, make_target  # noqa: E402
 from scripts.bench_alpha import card, median, timed  # noqa: E402
 
-SETTINGS = (("off", False), ("on", True))
+# (name, camera gradients on, intrinsics / tanfov requiring grad)
+SETTINGS = (("off", False, False), ("extrinsics", True, False), ("extrinsics+intrinsics", True, True))
 
 
 def _measure(step, dev, args):
-    out = {name: [] for name, _ in SETTINGS}
+    out = {name: [] for name, _, _ in SETTINGS}
     for _ in range(args.rounds):
-        for name, on in SETTINGS:
-            out[name].append(timed(lambda: step(on), args.steps, args.warmup))
+        for name, on, intr in SETTINGS:
+            out[name].append(timed(lambda: step(on, intr), args.steps, args.warmup))
     stages = {}
-    for name, on in SETTINGS:   # stage times in a pass of their own (profiling synchronises every stage)
+    for name, on, intr in SETTINGS:   # stage times in a pass of their own (profiling synchronises every stage)
         set_profiling(True, dev)
         ms = []
         for _ in range(args.steps):
-            step(on)
+            step(on, intr)
             torch.cuda.synchronize()
             ms.append(stage_ms(dev))
         set_profiling(False, dev)
@@ -53,12 +55,14 @@ def training_shape(args, dev):
     L = [st(n).clone().requires_grad_(True) for n in ("means", "covariances", "harmonics", "opacities")]
     ext = st("extrinsics").clone().requires_grad_(True)
     intr = st("intrinsics")
+    intr_g = intr.clone().requires_grad_(True)
     near, far = torch.full((b, v), 1.0, device=dev), torch.full((b, v), 100.0, device=dev)
     bg = torch.zeros(3, device=dev)
     tgt = make_target(b * v, *hw).to(dev).reshape(b, v, 3, *hw)
 
-    def step(on):
-        color, depth = decoder_forward(*L, ext, intr, near, far, hw, bg, depth_mode="depth", camera_gradients=on)
+    def step(on, with_intr):
+        color, depth = decoder_forward(*L, ext, intr_g if with_intr else intr, near, far, hw, bg, depth_mode="depth",
+                                       camera_gradients=on)
         (((color - tgt) ** 2).mean() + depth.mean()).backward()
 
     return {"b": b, "v": v, "gaussians_per_scene": int(L[0].shape[1]), "hw": list(hw), **_measure(step, dev, args)}
@@ -76,9 +80,11 @@ def c2(args, dev):
                 campos=vb.campos.to(dev).requires_grad_(True), bg=sc.background.to(dev), tanfov=vb.tanfov.to(dev),
                 view_scale=vb.scale.to(dev))
     bs = BatchSettings(image_height=256, image_width=256, sh_degree=4, **cams)
+    tan_g = cams["tanfov"].clone().requires_grad_(True)
 
-    def step(on):
-        out = rasterize_batch(bs._replace(camera_gradients=on), leaves[0], leaves[1], shs=leaves[2], cov3D_precomp=leaves[3])
+    def step(on, with_intr):
+        b = bs._replace(camera_gradients=on, tanfov=tan_g if with_intr else bs.tanfov)
+        out = rasterize_batch(b, leaves[0], leaves[1], shs=leaves[2], cov3D_precomp=leaves[3])
         (out[0] * W).sum().backward()
 
     return {"gaussians": int(leaves[0].shape[1]), "views": 8, "hw": [256, 256], **_measure(step, dev, args)}

@@ -468,6 +468,50 @@ GS_API int gs_pose_loss_backward(const GsPoseLossConfig *cfg, const GsPoseLossIn
                                  const float *dL_dL2, const GsPoseLossGrads *grads, void *scratch, void *stream);
 
 /*
+ * Plane-sweep cost volume = the parameter-free warp and correlation of PF3plat's DepthPredictorMultiView.forward
+ * (src/model/encoder/costvolume/depth_predictor_multiview.py:309-343, the tensor before the torch.cat), DESIGN.md 5.13:
+ *   cost[vb, d, p] = mean over the v-1 source views s of sum_c feat01[vb, c, p] warped_s[vb, c, d, p] / sqrt(C)
+ * in the reference's (v b) order (vb = vi * batch + bi), with prepare_feat_proj_data_lists' relative poses (v = 2 takes
+ * its special branch), the target view's intrinsics un-normalised row-wise, depth candidates
+ * 1 / (1/far + linspace(0, 1, D) (1/near - 1/far)), pixel-index coordinates, z clamped to >= 1e-3 and grid_sample's
+ * bilinear sampling (align_corners=True, zero padding per tap, every in-bounds tap multiplied in).
+ * Device pointers: features [batch, views, C, h, w] at the element strides feat_stride; intrinsics [batch, views, r, r]
+ * normalised, r = intrinsics_rows (3, or 4 read through [:3, :3]); extrinsics [batch, views, 4, 4]; near, far
+ * [batch, views]; all contiguous except features.  out_cost [views * batch, D, h, w].  The backward takes dL_dcost of
+ * that shape (contiguous) and writes dL_dfeatures contiguous [batch, views, C, h, w]; the cameras get no gradient (the
+ * reference builds the grid under no_grad).  Scratch: gs_costvolume_scratch_bytes(cfg, backward) bytes, 256-byte
+ * aligned, for the channel-last packing of the features, the camera block and, in the backward, the per-pixel gradient
+ * rows and the source accumulators.  The forward and the backward's feat01 role are deterministic; the source role
+ * adds float atomics unless flags has GS_COSTVOLUME_DETERMINISTIC, which makes it bit-reproducible (exact fixed-point
+ * accumulation, a non-finite or out-of-range term makes its element NaN) and needs (views-1) D h w < 2^21.
+ * No host synchronisation.
+ */
+enum { GS_COSTVOLUME_DETERMINISTIC = 1u };
+
+typedef struct GsCostVolumeConfig {
+    int32_t batch, views, channels, height, width; /* views >= 2, height, width >= 2 */
+    int32_t depth_candidates;                      /* D >= 1 */
+    int32_t intrinsics_rows;                       /* 3 or 4 */
+    uint32_t flags;                                /* GS_COSTVOLUME_* */
+    int64_t feat_stride[5];                        /* element strides of features [batch, views, C, h, w] */
+} GsCostVolumeConfig;
+
+typedef struct GsCostVolumeInputs {
+    const float *features, *intrinsics, *extrinsics, *near_, *far_;
+} GsCostVolumeInputs;
+
+typedef struct GsCostVolumeGrads {
+    const float *dL_dcost; /* in:  [views * batch, D, h, w] */
+    float *dL_dfeatures;   /* out: [batch, views, C, h, w] */
+} GsCostVolumeGrads;
+
+GS_API int64_t gs_costvolume_scratch_bytes(const GsCostVolumeConfig *cfg, int32_t backward); /* -1: invalid config */
+GS_API int gs_costvolume_forward(const GsCostVolumeConfig *cfg, const GsCostVolumeInputs *in, float *out_cost,
+                                 void *scratch, void *stream);
+GS_API int gs_costvolume_backward(const GsCostVolumeConfig *cfg, const GsCostVolumeInputs *in,
+                                  const GsCostVolumeGrads *grads, void *scratch, void *stream);
+
+/*
  * LPIPS-VGG = the `lpips` package's LPIPS(net="vgg", version="0.1"), spatial=False, as PF3plat's LossLpips
  * (src/loss/loss_lpips.py:55-59) and compute_lpips (src/evaluation/metrics.py:27-33) call it; forward and input
  * gradients (the weights are constants).  The weights are an input:

@@ -153,6 +153,23 @@ class GsPoseLossGrads(Structure):
     _fields_ = [(n, c_void_p) for n in ("dL_dT", "dL_ddepth", "dL_dxyz", "dL_dw", "dL_dconf")]
 
 
+GS_COSTVOLUME_DETERMINISTIC = 1
+
+
+class GsCostVolumeConfig(Structure):
+    _fields_ = [("batch", c_int32), ("views", c_int32), ("channels", c_int32), ("height", c_int32), ("width", c_int32),
+                ("depth_candidates", c_int32), ("intrinsics_rows", c_int32), ("flags", c_uint32),
+                ("feat_stride", c_int64 * 5)]
+
+
+class GsCostVolumeInputs(Structure):
+    _fields_ = [(n, c_void_p) for n in ("features", "intrinsics", "extrinsics", "near_", "far_")]
+
+
+class GsCostVolumeGrads(Structure):
+    _fields_ = [("dL_dcost", c_void_p), ("dL_dfeatures", c_void_p)]
+
+
 SYMBOLS = {
     "gs_abi_version": (c_int, []),
     "gs_last_error": (c_char_p, []),
@@ -204,6 +221,11 @@ SYMBOLS = {
     "gs_pose_loss_forward": (c_int, [POINTER(GsPoseLossConfig), POINTER(GsPoseLossInputs), c_void_p, c_void_p, c_void_p]),
     "gs_pose_loss_backward": (c_int, [POINTER(GsPoseLossConfig), POINTER(GsPoseLossInputs), c_void_p, c_void_p,
                                       POINTER(GsPoseLossGrads), c_void_p, c_void_p]),
+    "gs_costvolume_scratch_bytes": (c_int64, [POINTER(GsCostVolumeConfig), c_int32]),
+    "gs_costvolume_forward": (c_int, [POINTER(GsCostVolumeConfig), POINTER(GsCostVolumeInputs), c_void_p, c_void_p,
+                                      c_void_p]),
+    "gs_costvolume_backward": (c_int, [POINTER(GsCostVolumeConfig), POINTER(GsCostVolumeInputs),
+                                       POINTER(GsCostVolumeGrads), c_void_p, c_void_p]),
 }
 
 

@@ -2,7 +2,9 @@
 src/model/encoder/costvolume/depth_predictor_multiview.py: `prepare_feat_proj_data_lists` and
 `warp_with_pose_depth_candidates`, imported unmodified from a PF3plat checkout) with the correlation and mean lines of
 `DepthPredictorMultiView.forward` (:309-343) on small seeded cases, in float32 and in float64, and recording the cost
-volume and the autograd gradient of sum(cost * cotangent) with respect to the features.
+volume and the autograd gradient of sum(cost * cotangent) with respect to the features.  Cases added later draw from a
+generator of their own, after the earlier ones, so that regenerating the file reproduces every earlier array byte for
+byte.
 
 Needs a PF3plat checkout, named by $PF3PLAT_ROOT.  The module imports its U-Net (.ldm_unet.unet) at module level for
 the network around the op; that import is stubbed.  `coords_grid` casts its integer pixel grid to float32 with
@@ -124,6 +126,17 @@ def cases():
     c["features"][0, 1, 0, 3, 7] = np.inf
     c["features"][0, 1, 2, 6, 2] = -np.inf
     out["v2_nonfinite"] = c
+    # Past the kernels' first 256-channel pass, past poison word 0, and beyond four views.  These cases draw from their
+    # own generator, so the arrays of the cases above stay exactly as they were.
+    rng = np.random.default_rng(20261018)
+    c = make_case(rng, 1, 2, 300, 3, 4, 3)  # NaN at channel 290 of view 0, +Inf at 40 and -Inf at 256 of view 1
+    c["features"][0, 0, 290, 1, 1] = np.nan
+    c["features"][0, 1, 40, 1, 2] = np.inf
+    c["features"][0, 1, 256, 2, 1] = -np.inf
+    out["v2_c300_nonfinite"] = c
+    out["v5_b2_c130"] = make_case(rng, 2, 5, 130, 4, 5, 4, rows=4, near=(0.8, 1.5), far=(6.0, 12.0))
+    out["v8_c5_d3"] = make_case(rng, 1, 8, 5, 3, 3, 3, near=(0.8, 1.5), far=(6.0, 12.0))
+    out["v2_c257_d2"] = make_case(rng, 1, 2, 257, 3, 3, 2)  # second pass: one float4 chunk, three quarters padding
     return out
 
 

@@ -98,9 +98,25 @@ def test_golden_cases_reach_their_regimes():
     assert (np.abs(K[..., 0, 1]) > 0).all() and (np.abs(K[..., :2, 2] - 0.5) > 1e-3).any()
     assert CASES["v4_b3_c1_k4x4"]["intrinsics"].shape[-1] == 4
     assert len(np.unique(CASES["v2_skew_pp"]["near"])) == 4 and len(np.unique(CASES["v2_skew_pp"]["far"])) == 4
-    for name in ("v2_nonfinite",):
+    for name in ("v2_nonfinite", "v2_c300_nonfinite"):
         v = CASES[name]["value64"]
         assert np.isnan(v).any() and not np.isfinite(CASES[name]["grad64"]).all()
+    # The kernels hold 256 channels (64 float4 chunks) per pass; the poison mask has one 32-bit word per 32 channels.
+    shapes = {n: c["features"].shape for n, c in CASES.items()}  # [b, v, C, h, w]
+    cp4 = {n: (s[2] + 3) // 4 for n, s in shapes.items()}
+    assert {n for n, s in shapes.items() if s[2] > 256} == {"v2_c300_nonfinite", "v2_c257_d2"}
+    assert cp4["v2_c257_d2"] == 64 + 1  # the second pass is one chunk, three of its four channels padding
+    assert {n for n, s in shapes.items() if s[2] % 4 and cp4[n] > 1} >= {"v8_c5_d3", "v5_b2_c130", "v2_c257_d2"}
+    assert shapes["v5_b2_c130"][:2] == (2, 5) and CASES["v5_b2_c130"]["intrinsics"].shape[-1] == 4
+    assert shapes["v8_c5_d3"][1] == 8
+    # non-finite features at channels in poison words 1, 8 and 9, in both views, and non-finite gradients at each of
+    # those channels: in view 0 where it samples view 1's +-Inf, in view 1 where view 0's NaN reaches it
+    c = CASES["v2_c300_nonfinite"]
+    bad = {(int(i[1]), int(i[2])) for i in np.argwhere(~np.isfinite(c["features"]))}
+    assert bad == {(0, 290), (1, 40), (1, 256)}
+    assert {ch // 32 for _, ch in bad} == {1, 8, 9}
+    gbad = {(int(i[1]), int(i[2])) for i in np.argwhere(~np.isfinite(c["grad64"]))}
+    assert gbad == {(0, 40), (0, 256), (1, 290)}
 
 
 @pytest.fixture(scope="module")

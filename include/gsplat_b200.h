@@ -512,6 +512,69 @@ GS_API int gs_costvolume_backward(const GsCostVolumeConfig *cfg, const GsCostVol
                                   const GsCostVolumeGrads *grads, void *scratch, void *stream);
 
 /*
+ * The encoder's pose path between PnP and the networks that read the poses (DESIGN.md 5.14).  No host synchronisation.
+ *
+ * gs_pose_sync = PF3plat's camera_synchronization (src/flow_util.py:623-743) at its default arguments: N = 2 chains
+ * (camera_chaining); otherwise the float32 L of the confidence-weighted pairs, squared ten times in fp64, column block
+ * 0 divided by its mass, the rotation projected onto SO(3) (one-sided Jacobi), rounded to float32.  If the smallest
+ * mass over the whole batch is exactly 0, every scene is chained.  A scene whose L (as built, or its column block after
+ * the squarings) holds a non-finite value gets NaN in all its outputs and a NaN mass, which turns the batch fallback off.
+ * Device pointers: Ps [pairs, batch, 4, 4] in the order of pair_i / pair_j, confidence [pairs, batch] (may be NULL when
+ * views == 2), out [batch, views, 4, 4]; all contiguous float32.  Pairs (i, j) need 0 <= i, j < views, i != j, no
+ * repeat in either order, every view in some pair and (k, k+1) for every k < views - 1 (the chain).
+ * Scratch: gs_pose_sync_scratch_bytes(cfg) bytes, 256-byte aligned.  Bit-reproducible (no atomics).
+ */
+enum { GS_POSES_MAX_VIEWS = 16, GS_POSES_MAX_PAIRS = 120 };
+
+typedef struct GsPoseSyncConfig {
+    int32_t batch, views, pairs, reserved_;   /* 2 <= views <= 16, 1 <= pairs <= views (views - 1) / 2 */
+    int8_t pair_i[GS_POSES_MAX_PAIRS], pair_j[GS_POSES_MAX_PAIRS];
+} GsPoseSyncConfig;
+
+GS_API int64_t gs_pose_sync_scratch_bytes(const GsPoseSyncConfig *cfg); /* -1 for an invalid config */
+GS_API int gs_pose_sync(const GsPoseSyncConfig *cfg, const float *Ps, const float *confidence, float *out, void *scratch,
+                        void *stream);
+
+/*
+ * gs_refine_poses = encoder_costvolume.py:465-473 and the .inverse() of its result: x = pose_enc (view 0) or
+ * pose_enc + delta * gamma (views >= 1), R = r6d2mat(x[:6]) (F.normalize's max(|v|, 1e-12), rows b1, b2, b1 x b2),
+ * abspose = [R | x[6:9]; 0 0 0 1] and abspose_inv its general 4x4 inverse, fp64 inside.  A singular abspose gives a
+ * non-finite inverse.  Device pointers, contiguous float32: pose_enc, delta [batch, views, 9], gamma [1]; abspose,
+ * abspose_inv [batch, views, 4, 4].  The backward takes either cotangent (NULL = zero) and writes all three gradients;
+ * dL_dgamma is a fixed-order fp64 reduction in one CTA, so the backward is bit-reproducible.
+ */
+typedef struct GsRefinePosesConfig {
+    int32_t batch, views; /* views >= 1 */
+} GsRefinePosesConfig;
+
+typedef struct GsRefinePosesInputs {
+    const float *pose_enc, *delta, *gamma;
+} GsRefinePosesInputs;
+
+typedef struct GsRefinePosesGrads {
+    const float *dL_dabspose, *dL_dabspose_inv;       /* in:  [batch, views, 4, 4], either may be NULL */
+    float *dL_dpose_enc, *dL_ddelta, *dL_dgamma;      /* out: [batch, views, 9], [batch, views, 9], [1] */
+} GsRefinePosesGrads;
+
+GS_API int gs_refine_poses_forward(const GsRefinePosesConfig *cfg, const GsRefinePosesInputs *in, float *abspose,
+                                   float *abspose_inv, void *stream);
+GS_API int gs_refine_poses_backward(const GsRefinePosesConfig *cfg, const GsRefinePosesInputs *in,
+                                    const GsRefinePosesGrads *grads, void *stream);
+
+/*
+ * gs_plucker_rays = plucker_embedding(h, w, *get_world_rays(grid, abspose.inverse(), K)) (encoder_costvolume.py:387-392,
+ * :211-221): pixel centres ((x + 1/2) / w, (y + 1/2) / h), d = normalise(K^-1 [x, y, 1]) rotated by c2w with w = 0,
+ * origin o = c2w[:3, 3], out [(batch views), 6, h, w] = (d, o x d), fp64 inside.  abspose [batch, views, 4, 4] and
+ * intrinsics [batch, views, 3, 3] contiguous float32; out contiguous.
+ */
+typedef struct GsPluckerConfig {
+    int32_t batch, views, height, width;
+} GsPluckerConfig;
+
+GS_API int gs_plucker_rays(const GsPluckerConfig *cfg, const float *abspose, const float *intrinsics, float *out,
+                           void *stream);
+
+/*
  * LPIPS-VGG = the `lpips` package's LPIPS(net="vgg", version="0.1"), spatial=False, as PF3plat's LossLpips
  * (src/loss/loss_lpips.py:55-59) and compute_lpips (src/evaluation/metrics.py:27-33) call it; forward and input
  * gradients (the weights are constants).  The weights are an input:

@@ -8,7 +8,7 @@ from __future__ import annotations
 
 import ctypes
 import os
-from ctypes import POINTER, Structure, c_char_p, c_float, c_int, c_int32, c_int64, c_uint32, c_void_p
+from ctypes import POINTER, Structure, c_char_p, c_float, c_int, c_int8, c_int32, c_int64, c_uint32, c_void_p
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "csrc", "libgsplat_b200.so")
@@ -170,6 +170,31 @@ class GsCostVolumeGrads(Structure):
     _fields_ = [("dL_dcost", c_void_p), ("dL_dfeatures", c_void_p)]
 
 
+GS_POSES_MAX_VIEWS = 16
+GS_POSES_MAX_PAIRS = 120
+
+
+class GsPoseSyncConfig(Structure):
+    _fields_ = [("batch", c_int32), ("views", c_int32), ("pairs", c_int32), ("reserved_", c_int32),
+                ("pair_i", c_int8 * GS_POSES_MAX_PAIRS), ("pair_j", c_int8 * GS_POSES_MAX_PAIRS)]
+
+
+class GsRefinePosesConfig(Structure):
+    _fields_ = [("batch", c_int32), ("views", c_int32)]
+
+
+class GsRefinePosesInputs(Structure):
+    _fields_ = [(n, c_void_p) for n in ("pose_enc", "delta", "gamma")]
+
+
+class GsRefinePosesGrads(Structure):
+    _fields_ = [(n, c_void_p) for n in ("dL_dabspose", "dL_dabspose_inv", "dL_dpose_enc", "dL_ddelta", "dL_dgamma")]
+
+
+class GsPluckerConfig(Structure):
+    _fields_ = [("batch", c_int32), ("views", c_int32), ("height", c_int32), ("width", c_int32)]
+
+
 SYMBOLS = {
     "gs_abi_version": (c_int, []),
     "gs_last_error": (c_char_p, []),
@@ -226,6 +251,13 @@ SYMBOLS = {
                                       c_void_p]),
     "gs_costvolume_backward": (c_int, [POINTER(GsCostVolumeConfig), POINTER(GsCostVolumeInputs),
                                        POINTER(GsCostVolumeGrads), c_void_p, c_void_p]),
+    "gs_pose_sync_scratch_bytes": (c_int64, [POINTER(GsPoseSyncConfig)]),
+    "gs_pose_sync": (c_int, [POINTER(GsPoseSyncConfig), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "gs_refine_poses_forward": (c_int, [POINTER(GsRefinePosesConfig), POINTER(GsRefinePosesInputs), c_void_p, c_void_p,
+                                        c_void_p]),
+    "gs_refine_poses_backward": (c_int, [POINTER(GsRefinePosesConfig), POINTER(GsRefinePosesInputs),
+                                         POINTER(GsRefinePosesGrads), c_void_p]),
+    "gs_plucker_rays": (c_int, [POINTER(GsPluckerConfig), c_void_p, c_void_p, c_void_p, c_void_p]),
 }
 
 

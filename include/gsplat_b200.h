@@ -575,6 +575,73 @@ GS_API int gs_plucker_rays(const GsPluckerConfig *cfg, const float *abspose, con
                            void *stream);
 
 /*
+ * The encoder's depth glue between UniDepth and the networks and losses that read its output (DESIGN.md 5.15).  No host
+ * synchronisation, no atomics: every backward is a fixed-order gather and bit-reproducible.
+ *
+ * gs_depth_update = encoder_costvolume.py:265, :285-287 with get_scaleshift (:167-172) and the unprojections :304-307,
+ * :506-528: d0 = clamp(depth, near, far); s = the scale-shift head's channel 1 bilinearly upsampled (align_corners =
+ * False, PyTorch's source index) from the (grid_height, grid_width) feature grid to (height, width), clamped to
+ * [-5, 5]; depths = clamp(d0 + s, near, far), all in fp64 and rounded once; xyz = K^-1 [(x + 1/2) / w, (y + 1/2) / h,
+ * 1] depths (K^-1 in fp64).
+ * clamp propagates NaN.  Device pointers, contiguous float32: depth, depths [(batch views), 1, h, w]; scale_shift
+ * [batch, views, grid_height grid_width, 2] (channel 0 the scale, unused); intrinsics [batch, views, 3, 3]; near_,
+ * far_ [batch, views]; xyz [batch, views, 3, h, w].  The backward takes dL/ddepths and dL/dxyz (either may be NULL),
+ * masks them by both clamps (the gradient passes where lo <= x <= hi, a NaN passes nothing) and gathers them per
+ * feature-grid cell, one warp per cell, into dL/dscale_shift (channel 0 written as 0).
+ */
+typedef struct GsDepthUpdateConfig {
+    int32_t batch, views, height, width, grid_height, grid_width;
+} GsDepthUpdateConfig;
+
+typedef struct GsDepthUpdateInputs {
+    const float *depth, *scale_shift, *intrinsics, *near_, *far_;
+} GsDepthUpdateInputs;
+
+typedef struct GsDepthUpdateGrads {
+    const float *dL_ddepths, *dL_dxyz; /* in:  [(batch views), 1, h, w], [batch, views, 3, h, w]; either may be NULL */
+    float *dL_dscale_shift;            /* out: [batch, views, grid_height grid_width, 2] */
+} GsDepthUpdateGrads;
+
+GS_API int gs_depth_update_forward(const GsDepthUpdateConfig *cfg, const GsDepthUpdateInputs *in, float *depths,
+                                   float *xyz, void *stream);
+GS_API int gs_depth_update_backward(const GsDepthUpdateConfig *cfg, const GsDepthUpdateInputs *in,
+                                    const GsDepthUpdateGrads *grads, void *stream);
+
+/*
+ * gs_mono_cue = encoder_costvolume.py:292-298, the one-hot mono cue (forward only): depths [(batch views), 1, h, w]
+ * downsampled bilinearly by exactly 4 (h, w multiples of 4: taps 4i+1, 4i+2 at weight 1/2, in PyTorch's order), then
+ * the index of the first smallest |d - h_k| over GS_MONO_CUE_BINS hypotheses (a NaN difference counts as smallest, as
+ * in torch.argmin), written as a one-hot into out [(views batch), GS_MONO_CUE_BINS, h/4, w/4].  Every scene uses
+ * near_[0] and far_[0], read on the device: h_k = fl32(a + fl32(lin[k] fl32(B))), a = fl32(1 / far_[0]),
+ * B = (double)fl32(1 / near_[0]) - (double)a.  lin is a device array of GS_MONO_CUE_BINS floats holding the values
+ * of torch.linspace(0, 1, 128) on the CPU.
+ */
+enum { GS_MONO_CUE_BINS = 128 };
+
+typedef struct GsMonoCueConfig {
+    int32_t batch, views, height, width; /* height, width: the full-resolution frame, multiples of 4 */
+} GsMonoCueConfig;
+
+GS_API int gs_mono_cue(const GsMonoCueConfig *cfg, const float *depths, const float *near_, const float *far_,
+                       const float *lin, float *out, void *stream);
+
+/*
+ * gs_pdf_peak = depth_predictor_multiview.py:379-384: max over D of softmax over D of logits [items, D, h, w],
+ * i.e. 1 / sum_k exp(x_k - x_max), nearest-upsampled by the integer `upscale` into out [items, 1, h s, w s].  The
+ * forward also writes the per-pixel peak [items, h, w] and argmax [items, h, w] (ties to the lowest index) for the
+ * backward, which takes dL/dout, sums each pixel's s^2 cotangents in a fixed order into G and writes
+ * dL/dlogits_k = G p* (delta_{k, k*} - p_k), with p_k recomputed from the logits.
+ */
+typedef struct GsPdfPeakConfig {
+    int32_t items, depth_candidates, height, width, upscale;
+} GsPdfPeakConfig;
+
+GS_API int gs_pdf_peak_forward(const GsPdfPeakConfig *cfg, const float *logits, float *out, float *peak,
+                               int32_t *argmax, void *stream);
+GS_API int gs_pdf_peak_backward(const GsPdfPeakConfig *cfg, const float *logits, const float *peak,
+                                const int32_t *argmax, const float *dL_dout, float *dL_dlogits, void *stream);
+
+/*
  * LPIPS-VGG = the `lpips` package's LPIPS(net="vgg", version="0.1"), spatial=False, as PF3plat's LossLpips
  * (src/loss/loss_lpips.py:55-59) and compute_lpips (src/evaluation/metrics.py:27-33) call it; forward and input
  * gradients (the weights are constants).  The weights are an input:

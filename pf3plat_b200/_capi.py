@@ -195,6 +195,29 @@ class GsPluckerConfig(Structure):
     _fields_ = [("batch", c_int32), ("views", c_int32), ("height", c_int32), ("width", c_int32)]
 
 
+class GsDepthUpdateConfig(Structure):
+    _fields_ = [(n, c_int32) for n in ("batch", "views", "height", "width", "grid_height", "grid_width")]
+
+
+class GsDepthUpdateInputs(Structure):
+    _fields_ = [(n, c_void_p) for n in ("depth", "scale_shift", "intrinsics", "near_", "far_")]
+
+
+class GsDepthUpdateGrads(Structure):
+    _fields_ = [(n, c_void_p) for n in ("dL_ddepths", "dL_dxyz", "dL_dscale_shift")]
+
+
+GS_MONO_CUE_BINS = 128
+
+
+class GsMonoCueConfig(Structure):
+    _fields_ = [(n, c_int32) for n in ("batch", "views", "height", "width")]
+
+
+class GsPdfPeakConfig(Structure):
+    _fields_ = [(n, c_int32) for n in ("items", "depth_candidates", "height", "width", "upscale")]
+
+
 SYMBOLS = {
     "gs_abi_version": (c_int, []),
     "gs_last_error": (c_char_p, []),
@@ -258,6 +281,14 @@ SYMBOLS = {
     "gs_refine_poses_backward": (c_int, [POINTER(GsRefinePosesConfig), POINTER(GsRefinePosesInputs),
                                          POINTER(GsRefinePosesGrads), c_void_p]),
     "gs_plucker_rays": (c_int, [POINTER(GsPluckerConfig), c_void_p, c_void_p, c_void_p, c_void_p]),
+    "gs_depth_update_forward": (c_int, [POINTER(GsDepthUpdateConfig), POINTER(GsDepthUpdateInputs), c_void_p, c_void_p,
+                                        c_void_p]),
+    "gs_depth_update_backward": (c_int, [POINTER(GsDepthUpdateConfig), POINTER(GsDepthUpdateInputs),
+                                         POINTER(GsDepthUpdateGrads), c_void_p]),
+    "gs_mono_cue": (c_int, [POINTER(GsMonoCueConfig), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "gs_pdf_peak_forward": (c_int, [POINTER(GsPdfPeakConfig), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "gs_pdf_peak_backward": (c_int, [POINTER(GsPdfPeakConfig), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                     c_void_p]),
 }
 
 

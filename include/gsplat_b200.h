@@ -642,6 +642,72 @@ GS_API int gs_pdf_peak_backward(const GsPdfPeakConfig *cfg, const float *logits,
                                 const int32_t *argmax, const float *dL_dout, float *dL_dlogits, void *stream);
 
 /*
+ * The Gaussian head between the depth predictor's two output convolutions and the decoder (DESIGN.md 5.16), for
+ * gaussians_per_pixel = num_surfaces = 1:
+ *   depth_predictor_multiview.py:397-415   the (v b) c h w -> b v (h w) c rearrange of to_gaussians' output, the split
+ *                                          of to_disparity's output and the sigmoid of its channel 1
+ *   encoder_costvolume.py:509-518          pixel centres ((i + 1/2) / w, (j + 1/2) / h) moved by
+ *                                          (sigmoid(raw[0:2]) - 1/2) (1/w, 1/h), in float32 as the reference rounds it
+ *   encoder_costvolume.py:529-540          the adapter on raw[2:] with views 0 and V - 1 of depths, c2w and intrinsics
+ *                                          (gaussian_adapter.py:60-92; K^-1 and get_scale_multiplier in fp64 per camera)
+ *   encoder_costvolume.py:174-187, :534    opacities = 0.5 (1 - (1 - q) + q), q = sigmoid(density), / gpp = 1
+ *   encoder_costvolume.py:556-573          every output in b (v r srf spp) order: slot 0's pixels row-major, then
+ *                                          slot 1's (the context's view V - 1), G = 2 h w Gaussians per scene
+ * One launch forward, two backward; no host synchronisation, no float atomics (bit-reproducible).
+ */
+typedef struct GsGaussianHeadConfig {
+    int32_t batch;      /* b; 2 batch <= 65535 cameras */
+    int32_t views;      /* V >= 2: the context views of depths, c2w and intrinsics (encoder_costvolume.py:530-533) */
+    int32_t height;     /* h of the depth predictor's full-resolution output */
+    int32_t width;      /* w */
+    int32_t d_sh;       /* (sh_degree + 1)^2 <= 25 (gaussian_adapter.py:113-115) */
+    uint32_t flags;     /* 0 */
+    float scale_min;    /* GaussianAdapterCfg.gaussian_scale_min (gaussian_adapter.py:63) */
+    float scale_max;    /* GaussianAdapterCfg.gaussian_scale_max (gaussian_adapter.py:64) */
+    float eps;          /* GaussianAdapter.forward's eps, 1e-8 (gaussian_adapter.py:57, :73) */
+    int32_t reserved_;
+} GsGaussianHeadConfig;
+
+typedef struct GsGaussianHeadInputs { /* device, contiguous float32 */
+    const float *raw_gaussians;  /* [(2 batch), 9 + 3 d_sh, h, w]: to_gaussians' output (depth_predictor_multiview.py:397),
+                                    (v b) order; channels: offset xy 2 | scales 3 | quaternion xyzw 4 | sh (xyz, d_sh) */
+    const float *density_logits; /* [(2 batch), 2, h, w]: to_disparity's output (:403); channel 1 the raw density */
+    const float *depths;         /* [(batch views), 1, h, w]: depths_final (encoder_costvolume.py:528) */
+    const float *c2w;            /* [batch, views, 4, 4]: refine_sync_abspose.inverse() (:530) */
+    const float *intrinsics;     /* [batch, views, 3, 3] normalised (:531) */
+    const float *sh_rotation;    /* [batch, 2, d_sh, d_sh] block-diagonal Wigner-D of slot 0 / 1's c2w[:3, :3] after the
+                                    rotation guard (misc/sh_rotation.py:21-34), or NULL = identity */
+    const float *sh_mask;        /* [d_sh] (gaussian_adapter.py:39-46) */
+} GsGaussianHeadInputs;
+
+typedef struct GsGaussianHeadOutputs { /* the four fields of model/types.py's Gaussians (encoder_costvolume.py:556-573) */
+    float *means;       /* [batch, 2 h w, 3] */
+    float *covariances; /* [batch, 2 h w, 3, 3] */
+    float *harmonics;   /* [batch, 2 h w, d_sh, 3]: the reference's (3, d_sh) is the transposed view */
+    float *opacities;   /* [batch, 2 h w] */
+} GsGaussianHeadOutputs;
+
+typedef struct GsGaussianHeadOutGrads { /* incoming gradients, shaped as GsGaussianHeadOutputs; NULL = zero */
+    const float *means, *covariances, *harmonics, *opacities;
+} GsGaussianHeadOutGrads;
+
+typedef struct GsGaussianHeadInGrads { /* written, not accumulated; any may be NULL */
+    float *raw_gaussians;  /* [(2 batch), 9 + 3 d_sh, h, w] */
+    float *density_logits; /* [(2 batch), 2, h, w]: channel 0 (delta_disps, unused by :404) gets 0 */
+    float *depths;         /* [(batch views), 1, h, w]: views 1 .. V - 2 get 0 */
+    float *c2w;            /* [batch, views, 4, 4]: through the means only (gaussian_adapter.py:81 detaches the rotation
+                              elsewhere); row 3 and views 1 .. V - 2 get 0 */
+    void *scratch;         /* gs_gaussian_head_scratch_bytes(cfg) bytes, 16-byte aligned: required with c2w */
+} GsGaussianHeadInGrads;
+
+GS_API int64_t gs_gaussian_head_scratch_bytes(const GsGaussianHeadConfig *cfg); /* -1 for an invalid config */
+GS_API int gs_gaussian_head_forward(const GsGaussianHeadConfig *cfg, const GsGaussianHeadInputs *in,
+                                    const GsGaussianHeadOutputs *out, void *stream);
+GS_API int gs_gaussian_head_backward(const GsGaussianHeadConfig *cfg, const GsGaussianHeadInputs *in,
+                                     const GsGaussianHeadOutGrads *gout, const GsGaussianHeadInGrads *gin,
+                                     void *stream);
+
+/*
  * LPIPS-VGG = the `lpips` package's LPIPS(net="vgg", version="0.1"), spatial=False, as PF3plat's LossLpips
  * (src/loss/loss_lpips.py:55-59) and compute_lpips (src/evaluation/metrics.py:27-33) call it; forward and input
  * gradients (the weights are constants).  The weights are an input:

@@ -218,6 +218,28 @@ class GsPdfPeakConfig(Structure):
     _fields_ = [(n, c_int32) for n in ("items", "depth_candidates", "height", "width", "upscale")]
 
 
+
+class GsGaussianHeadConfig(Structure):
+    _fields_ = [(n, c_int32) for n in ("batch", "views", "height", "width", "d_sh")] + [
+        ("flags", c_uint32), ("scale_min", c_float), ("scale_max", c_float), ("eps", c_float), ("reserved_", c_int32)]
+
+
+class GsGaussianHeadInputs(Structure):
+    _fields_ = [(n, c_void_p) for n in ("raw_gaussians", "density_logits", "depths", "c2w", "intrinsics", "sh_rotation",
+                                        "sh_mask")]
+
+
+class GsGaussianHeadOutputs(Structure):
+    _fields_ = [(n, c_void_p) for n in ("means", "covariances", "harmonics", "opacities")]
+
+
+class GsGaussianHeadOutGrads(Structure):
+    _fields_ = [(n, c_void_p) for n in ("means", "covariances", "harmonics", "opacities")]
+
+
+class GsGaussianHeadInGrads(Structure):
+    _fields_ = [(n, c_void_p) for n in ("raw_gaussians", "density_logits", "depths", "c2w", "scratch")]
+
 SYMBOLS = {
     "gs_abi_version": (c_int, []),
     "gs_last_error": (c_char_p, []),
@@ -289,6 +311,11 @@ SYMBOLS = {
     "gs_pdf_peak_forward": (c_int, [POINTER(GsPdfPeakConfig), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "gs_pdf_peak_backward": (c_int, [POINTER(GsPdfPeakConfig), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                      c_void_p]),
+    "gs_gaussian_head_scratch_bytes": (c_int64, [POINTER(GsGaussianHeadConfig)]),
+    "gs_gaussian_head_forward": (c_int, [POINTER(GsGaussianHeadConfig), POINTER(GsGaussianHeadInputs),
+                                         POINTER(GsGaussianHeadOutputs), c_void_p]),
+    "gs_gaussian_head_backward": (c_int, [POINTER(GsGaussianHeadConfig), POINTER(GsGaussianHeadInputs),
+                                          POINTER(GsGaussianHeadOutGrads), POINTER(GsGaussianHeadInGrads), c_void_p]),
 }
 
 

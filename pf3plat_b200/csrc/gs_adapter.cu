@@ -19,6 +19,7 @@
 // leaves by one bulk TMA store, so both big streams are fully coalesced; the backward mirrors it (gradient of the
 // harmonics in by TMA, gradient of the raw rows out by TMA).  HBM-bound: 328 + 12 B in, 300 + 76 B out per Gaussian.
 #include "gs_common.cuh"
+#include "gs_adapter_math.cuh"
 
 namespace {
 
@@ -39,18 +40,7 @@ struct AdapterInGrads {
     float *cam_partial;  // deterministic mode: [V][CTAs per camera][AD_CAM_SUMS] per-CTA sums (see k_adapter_bwd)
 };
 
-constexpr int AD_THREADS = 128;
 constexpr int AD_CAM_SUMS = 22;  // per-camera sums of the backward: dKinv 9 | dC 9 | dt 3 | dmultiplier 1
-constexpr int AD_MAX_DSH = 25;
-constexpr float AD_QUAT_EPS = 1e-8f;  // quaternion_to_matrix's own eps (PF3plat's src/model/encoder/common/gaussians.py:10)
-
-struct AdHdr {
-    float kinv[9], rot[9], t[3], mult;
-    float mask[AD_MAX_DSH];
-    float red[AD_THREADS / 32][24];
-    uint64_t bar;
-};
-constexpr int AD_HDR_BYTES = (sizeof(AdHdr) + 127) / 128 * 128;
 
 __device__ __forceinline__ void load_camera(const AdapterArgs &a, int v, AdHdr *h) {
     const int tid = threadIdx.x;
@@ -63,63 +53,6 @@ __device__ __forceinline__ void load_camera(const AdapterArgs &a, int v, AdHdr *
         h->mult = a.mult[v];
     }
     if (tid >= 32 && tid < 32 + a.d_sh) h->mask[tid - 32] = a.sh_mask[tid - 32];
-}
-
-// The geometry part of one Gaussian (everything but the harmonics); kept by the backward for its chain rule.
-struct AdGeom {
-    float dc[3], inv_n;   // camera-space unit direction, 1 / |Kinv (x,y,1)|
-    float dw[3];          // world-space direction
-    float sg[3], s0[3], s[3];
-    float q[4], nq, A;    // normalised quaternion (i,j,k,r), |raw quaternion|, two_s
-    float Rq[9];
-};
-
-__device__ __forceinline__ void adapter_geometry(const AdHdr &h, float x, float y, float z, const float *sraw, const float *qraw,
-                                                 float smin, float smax, float eps, AdGeom &g) {
-    float u[3];
-#pragma unroll
-    for (int i = 0; i < 3; i++) u[i] = h.kinv[i * 3] * x + h.kinv[i * 3 + 1] * y + h.kinv[i * 3 + 2];
-    g.inv_n = 1.0f / sqrtf(u[0] * u[0] + u[1] * u[1] + u[2] * u[2]);
-#pragma unroll
-    for (int i = 0; i < 3; i++) g.dc[i] = u[i] * g.inv_n;
-#pragma unroll
-    for (int i = 0; i < 3; i++) g.dw[i] = h.rot[i * 3] * g.dc[0] + h.rot[i * 3 + 1] * g.dc[1] + h.rot[i * 3 + 2] * g.dc[2];
-#pragma unroll
-    for (int k = 0; k < 3; k++) {
-        g.sg[k] = 1.0f / (1.0f + expf(-sraw[k]));
-        g.s0[k] = smin + (smax - smin) * g.sg[k];
-        g.s[k] = g.s0[k] * z * h.mult;
-    }
-    g.nq = sqrtf(qraw[0] * qraw[0] + qraw[1] * qraw[1] + qraw[2] * qraw[2] + qraw[3] * qraw[3]);
-    const float inv = 1.0f / (g.nq + eps);
-#pragma unroll
-    for (int k = 0; k < 4; k++) g.q[k] = qraw[k] * inv;
-    const float i = g.q[0], j = g.q[1], k = g.q[2], r = g.q[3];
-    g.A = 2.0f / (i * i + j * j + k * k + r * r + AD_QUAT_EPS);
-    const float A = g.A;
-    g.Rq[0] = 1.0f - A * (j * j + k * k); g.Rq[1] = A * (i * j - k * r);        g.Rq[2] = A * (i * k + j * r);
-    g.Rq[3] = A * (i * j + k * r);        g.Rq[4] = 1.0f - A * (i * i + k * k); g.Rq[5] = A * (j * k - i * r);
-    g.Rq[6] = A * (i * k - j * r);        g.Rq[7] = A * (j * k + i * r);        g.Rq[8] = 1.0f - A * (i * i + j * j);
-}
-
-// N = C Rq diag(s): the world-space covariance is N N^T
-__device__ __forceinline__ void adapter_factor(const AdHdr &h, const AdGeom &g, float *N) {
-    float M[9];
-#pragma unroll
-    for (int i = 0; i < 3; i++)
-#pragma unroll
-        for (int k = 0; k < 3; k++) M[i * 3 + k] = g.Rq[i * 3 + k] * g.s[k];
-#pragma unroll
-    for (int i = 0; i < 3; i++)
-#pragma unroll
-        for (int k = 0; k < 3; k++)
-            N[i * 3 + k] = h.rot[i * 3] * M[k] + h.rot[i * 3 + 1] * M[3 + k] + h.rot[i * 3 + 2] * M[6 + k];
-}
-
-__device__ __forceinline__ int isqrt_small(int n) {
-    int r = 0;
-    while ((r + 1) * (r + 1) <= n) r++;
-    return r;
 }
 
 __global__ void __launch_bounds__(AD_THREADS) k_adapter_fwd(const AdapterArgs a, const AdapterOut o) {
@@ -181,29 +114,9 @@ __global__ void __launch_bounds__(AD_THREADS) k_adapter_fwd(const AdapterArgs a,
         const float *sh = row + 7;
         if (a.sh_rot) {
             const float *D = a.sh_rot + (size_t)v * a.d_sh * a.d_sh;  // same address across the CTA: L1 broadcast
-            const int degs = isqrt_small(a.d_sh);
-            for (int l = 0; l < degs; l++) {
-                const int b = l * l, w = 2 * l + 1;
-                for (int i = 0; i < w; i++) {
-                    float acc0 = 0.f, acc1 = 0.f, acc2 = 0.f;
-                    for (int j = 0; j < w; j++) {
-                        const float d = D[(b + i) * a.d_sh + b + j] * h->mask[b + j];
-                        acc0 = fmaf(d, sh[b + j], acc0);
-                        acc1 = fmaf(d, sh[a.d_sh + b + j], acc1);
-                        acc2 = fmaf(d, sh[2 * a.d_sh + b + j], acc2);
-                    }
-                    out[(b + i) * 3] = acc0;
-                    out[(b + i) * 3 + 1] = acc1;
-                    out[(b + i) * 3 + 2] = acc2;
-                }
-            }
+            GS_SH_ROTATE_FWD(D, a.d_sh, h->mask, sh, out);
         } else {
-            for (int d = 0; d < a.d_sh; d++) {
-                const float m = h->mask[d];
-                out[d * 3] = sh[d] * m;
-                out[d * 3 + 1] = sh[a.d_sh + d] * m;
-                out[d * 3 + 2] = sh[2 * a.d_sh + d] * m;
-            }
+            GS_SH_MASK_FWD(a.d_sh, h->mask, sh, out);
         }
     }
     float *dst = o.harm + first * HS;
@@ -381,30 +294,9 @@ k_adapter_bwd(const AdapterArgs a, const AdapterOutGrads go, const AdapterInGrad
             const float *gh = gh_s + (size_t)tid * HS;
             if (a.sh_rot) {
                 const float *D = a.sh_rot + (size_t)v * a.d_sh * a.d_sh;
-                const int degs = isqrt_small(a.d_sh);
-                for (int l = 0; l < degs; l++) {
-                    const int b = l * l, w = 2 * l + 1;
-                    for (int j = 0; j < w; j++) {
-                        float acc0 = 0.f, acc1 = 0.f, acc2 = 0.f;
-                        for (int i = 0; i < w; i++) {
-                            const float d = D[(b + i) * a.d_sh + b + j];
-                            acc0 = fmaf(d, gh[(b + i) * 3], acc0);
-                            acc1 = fmaf(d, gh[(b + i) * 3 + 1], acc1);
-                            acc2 = fmaf(d, gh[(b + i) * 3 + 2], acc2);
-                        }
-                        const float m = h->mask[b + j];
-                        dsh[b + j] = acc0 * m;
-                        dsh[a.d_sh + b + j] = acc1 * m;
-                        dsh[2 * a.d_sh + b + j] = acc2 * m;
-                    }
-                }
+                GS_SH_ROTATE_BWD(D, a.d_sh, h->mask, gh, dsh);
             } else {
-                for (int d = 0; d < a.d_sh; d++) {
-                    const float m = h->mask[d];
-                    dsh[d] = gh[d * 3] * m;
-                    dsh[a.d_sh + d] = gh[d * 3 + 1] * m;
-                    dsh[2 * a.d_sh + d] = gh[d * 3 + 2] * m;
-                }
+                GS_SH_MASK_BWD(a.d_sh, h->mask, gh, dsh);
             }
         }
     }

@@ -281,7 +281,8 @@ k_adapter_bwd(const AdapterArgs a, const AdapterOutGrads go, const AdapterInGrad
             // q = qraw / (|qraw| + eps)
             const float inv = 1.0f / (g.nq + a.eps);
             const float dotq = dq[0] * qraw[0] + dq[1] * qraw[1] + dq[2] * qraw[2] + dq[3] * qraw[3];
-            const float radial = dotq * inv * inv / g.nq;
+            // d|q|/dq = q / |q| is 0/0 at a zero (or fully underflowed) raw quaternion: 0 there, as torch's norm
+            const float radial = g.nq == 0.f ? 0.f : dotq * inv * inv / g.nq;
 #pragma unroll
             for (int m = 0; m < 4; m++) drow[3 + m] = dq[m] * inv - qraw[m] * radial;
         }

@@ -287,7 +287,8 @@ k_head_bwd(const HeadArgs a, const HeadOutGrads go, const HeadInGrads gi_) {
             const float *qraw = r + 5;
             const float inv = 1.0f / (g.nq + a.eps);
             const float dotq = dq[0] * qraw[0] + dq[1] * qraw[1] + dq[2] * qraw[2] + dq[3] * qraw[3];
-            const float radial = dotq * inv * inv / g.nq;
+            // d|q|/dq = q / |q| is 0/0 at a zero (or fully underflowed) raw quaternion: 0 there, as torch's norm
+            const float radial = g.nq == 0.f ? 0.f : dotq * inv * inv / g.nq;
 #pragma unroll
             for (int m = 0; m < 4; m++) drow[5 + m] = dq[m] * inv - qraw[m] * radial;
         }

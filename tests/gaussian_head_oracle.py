@@ -28,15 +28,15 @@ def sh_rotation(c2w, d_sh):
 
 def head(raw, logits, depths, c2w, K, sh_degree, sh_rot=None, smin=SCALE_MIN, smax=SCALE_MAX, eps=1e-8):
     """float64 torch tensors (leaves may require grad) -> dict of means [b, G, 3], covariances [b, G, 3, 3], harmonics
-    [b, G, 3, d_sh], opacities [b, G], G = 2 h w"""
+    [b, G, 3, d_sh], opacities [b, G], G = 2 h w.  float32 tensors give the same statements in float32."""
     b, V = c2w.shape[:2]
     C, h, w = raw.shape[1:]
-    hw = h * w
+    hw, dt = h * w, raw.dtype
     r = raw.reshape(2, b, C, hw).permute(1, 0, 3, 2)                    # b v (h w) c
-    u = (torch.arange(w, dtype=torch.float64) + 0.5) / w
-    v = (torch.arange(h, dtype=torch.float64) + 0.5) / h
+    u = (torch.arange(w, dtype=dt) + 0.5) / w
+    v = (torch.arange(h, dtype=dt) + 0.5) / h
     grid = torch.stack(torch.meshgrid(u, v, indexing="xy"), -1).reshape(hw, 2)
-    ps = torch.tensor(1.0 / np.array([w, h], np.float32), dtype=torch.float64)
+    ps = torch.tensor(1.0 / np.array([w, h], np.float32), dtype=dt)
     xy = grid + (r[..., :2].sigmoid() - 0.5) * ps                          # [b, 2, hw, 2]
     sel = (0, V - 1)
     ext = c2w[:, sel][:, :, None]
@@ -51,7 +51,7 @@ def head(raw, logits, depths, c2w, K, sh_degree, sh_rot=None, smin=SCALE_MIN, sm
     multiplier = adapter_oracle.get_scale_multiplier(intr, ps)
     scales = scales * dep[..., None] * multiplier[..., None]
     rotations = rotations / (rotations.norm(dim=-1, keepdim=True) + eps)
-    sh = sh.reshape(*sh.shape[:-1], 3, d_sh) * adapter_oracle.sh_mask(sh_degree).to(torch.float64)
+    sh = sh.reshape(*sh.shape[:-1], 3, d_sh) * adapter_oracle.sh_mask(sh_degree).to(dt)
     rot = ext[..., :3, :3].detach()
     cov = rot @ adapter_oracle.build_covariance(scales, rotations) @ rot.transpose(-1, -2)
     origins, directions = adapter_oracle.get_world_rays(xy, ext, intr)
@@ -85,3 +85,14 @@ def run(case, cot=None):
     loss = sum((torch.tensor(np.asarray(cot[k], np.float64)) * out[k]).sum() for k in OUTPUTS)
     loss.backward()
     return vals, {k: t[k].grad.numpy() for k in INPUTS}
+
+
+def values32(case):
+    """the same statements in float32, as the reference runs them: the yardstick for how far float32 alone lands from
+    fp64 where a quantity is ill-conditioned (covariance entries that cancel between large scales)"""
+    deg = int(case["sh_degree"])
+    t = {k: torch.tensor(np.asarray(case[k]), dtype=torch.float32) for k in INPUTS}
+    K = torch.tensor(np.asarray(case["K"]), dtype=torch.float32)
+    sh = sh_rotation(case["c2w"], (deg + 1) ** 2).float() if deg > 0 else None
+    out = head(t["raw"], t["logits"], t["depths"], t["c2w"], K, deg, sh)
+    return {k: out[k].numpy() for k in OUTPUTS}

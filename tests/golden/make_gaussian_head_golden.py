@@ -10,7 +10,9 @@
 - the autograd gradients into raw, logits, depths and c2w of sum_k <cot_k, out_k> for random cotangents.
 All statements are taken from the method bodies by line number with `ast`.  To keep the record small, the inputs lie on
 coarse lattices, the cotangents are small integers, and the harmonics and dL/draw are recorded on a sample of the pixels
-that holds every non-finite or saturating input (`sample_pixels`); every other value and gradient is recorded in full.
+that holds every non-finite, saturating or degenerate input (`sample_pixels`); every other value and gradient is recorded
+in full.  Cases added later draw from seeds of their own, so that regenerating the file reproduces every earlier array
+byte for byte.
 Usage:  PF3PLAT_ROOT=<PF3plat checkout> python tests/golden/make_gaussian_head_golden.py
 """
 import ast
@@ -73,7 +75,7 @@ def load_reference():
     return adapter_mod, proj, typ, pred_code, enc_code, ns["map_pdf_to_opacity"]
 
 
-def make_case(seed, b, V, h, w, deg, improper=False, nan_c2w=False, extremes=False):
+def make_case(seed, b, V, h, w, deg, improper=False, nan_c2w=False, extremes=False, degenerate=()):
     rng = np.random.default_rng(seed)
     g = torch.Generator().manual_seed(seed)
     d_sh = (deg + 1) ** 2
@@ -100,6 +102,18 @@ def make_case(seed, b, V, h, w, deg, improper=False, nan_c2w=False, extremes=Fal
         raw[0, 3, h - 1, 0] = np.nan
         logits[0, 1, 0, :3] = [60.0, -60.0, 1e4]
         logits[1, 0, 1, 1] = np.nan  # channel 0 is discarded: no effect anywhere
+    # degenerate Gaussians, each (kind, conv item, pixel row, pixel col) or (kind, scene, view, row, col) for "depth":
+    # an exactly zero raw quaternion (|q| = 0, the norm's gradient 0/0), one whose float32 squares underflow to 0, a
+    # zero depth (zero scales, a covariance of 0)
+    for kind, *at in degenerate:
+        if kind == "zero_quat":
+            raw[at[0], 5:9, at[1], at[2]] = 0.0
+        elif kind == "tiny_quat":
+            raw[at[0], 5:9, at[1], at[2]] = [1e-25, -2e-25, 3e-25, 1e-25]
+        elif kind == "depth":
+            depths[at[0] * V + at[1], 0, at[2], at[3]] = 0.0
+        else:
+            raise ValueError(kind)
     f32 = lambda a: np.asarray(a, np.float32)  # noqa: E731
     case = {"raw": f32(raw), "logits": f32(logits), "depths": f32(depths), "c2w": f32(c2w), "K": f32(K),
             "sh_degree": np.int64(deg)}
@@ -121,6 +135,13 @@ def cases():
         "b2_v3_4x5_d25_improper": make_case(6, 2, 3, 4, 5, 4, improper=True),
         "b2_v2_4x4_d9_nan_c2w": make_case(7, 2, 2, 4, 4, 2, nan_c2w=True),
         "b1_v3_5x6_d25_extremes": make_case(8, 1, 3, 5, 6, 4, extremes=True),
+        # Cases added later: each draws from a seed of its own, so the arrays of the cases above stay byte for byte
+        # as they were.  Five and six views (three and four middle views), and the degenerate Gaussians of make_case
+        # in different scenes and slots: conv item s b + bi is slot s of scene bi.
+        "b2_v5_6x7_d16_degenerate": make_case(9, 2, 5, 6, 7, 3, degenerate=(
+            ("zero_quat", 0, 1, 2), ("tiny_quat", 3, 4, 5), ("depth", 1, 0, 2, 6), ("depth", 0, 4, 5, 0))),
+        "b3_v6_3x5_d25_degenerate": make_case(10, 3, 6, 3, 5, 4, degenerate=(
+            ("zero_quat", 4, 0, 0), ("tiny_quat", 2, 2, 4), ("zero_quat", 1, 1, 3), ("depth", 2, 5, 1, 1))),
     }
 
 
@@ -181,7 +202,17 @@ def sample_pixels(case):
     for a in (case["raw"], case["logits"]):
         bad = ~np.isfinite(a) | (np.abs(a) >= 15)
         pix |= {int(i) for i in np.flatnonzero(bad.any(axis=(0, 1)))}
+    pix |= {int(i) for i in np.flatnonzero(degenerate_pixels(case))}
     return np.array(sorted(pix), np.int64)
+
+
+def degenerate_pixels(case):
+    """[h w] bool: pixels whose raw quaternion has a float32 norm of 0 (exactly zero or underflowing) in some item, or
+    whose depth is 0 in some view"""
+    h, w = case["raw"].shape[-2:]
+    q = case["raw"][:, 5:9].astype(np.float32)
+    nq = np.sqrt((q * q).sum(1, dtype=np.float32))
+    return ((nq == 0).any(0) | (case["depths"][:, 0] == 0).any(0)).reshape(h * w)
 
 
 def at_sample(case, pix, key, a):

@@ -2,6 +2,7 @@
 (tests/golden/gaussian_head.npz, made by tests/golden/make_gaussian_head_golden.py) and against central finite
 differences; the C ABI's new structs against the header; refusals that need no device."""
 import ctypes
+import hashlib
 import os
 import subprocess
 
@@ -62,7 +63,7 @@ def test_golden_cases_reach_their_regimes():
     degs = {int(Z[f"{n}/sh_degree"]) for n in NAMES}
     assert degs == {0, 1, 2, 3, 4}
     views = {Z[f"{n}/c2w"].shape[1] for n in NAMES}
-    assert views == {2, 3, 4} and {Z[f"{n}/c2w"].shape[0] for n in NAMES} == {1, 2, 3}
+    assert views == {2, 3, 4, 5, 6} and {Z[f"{n}/c2w"].shape[0] for n in NAMES} == {1, 2, 3}
     assert any(Z[f"{n}/raw"].shape[-2] == 1 for n in NAMES) and any(Z[f"{n}/raw"].shape[-1] % 4 for n in NAMES)
     # the improper rotation fails the guard: every camera rotates by the identity, so harmonics are the masked raw
     imp = case("b2_v3_4x5_d25_improper")
@@ -85,6 +86,60 @@ def test_golden_cases_reach_their_regimes():
     pix = set(Z["b1_v3_5x6_d25_extremes/pix"].tolist())
     bad = (~np.isfinite(e["raw"]) | (np.abs(e["raw"]) >= 15)).any(axis=(0, 1)).reshape(-1)
     assert set(np.flatnonzero(bad).tolist()) <= pix and len(pix) >= 8
+    # the degenerate cases: two or more scenes, five and six views, and in different scenes or slots an exactly zero
+    # raw quaternion, one whose float32 squares underflow (|q| = 0 in float32, not in fp64) and a zero depth, each at a
+    # recorded pixel; the gradients there are finite, and exactly 0 on the zero quaternion
+    seen = {"zero": set(), "tiny": set(), "depth": set()}
+    for name in ("b2_v5_6x7_d16_degenerate", "b3_v6_3x5_d25_degenerate"):
+        c = case(name)
+        b, V = c["c2w"].shape[:2]
+        h, w = c["raw"].shape[-2:]
+        assert b >= 2 and V >= 5
+        pix = set(Z[f"{name}/pix"].tolist())
+        q = c["raw"][:, 5:9].reshape(2 * b, 4, h * w)
+        zero = (q == 0).all(1)
+        tiny = ~zero & ((q * q).sum(1, dtype=np.float32) == 0) & (np.abs(q.astype(np.float64)).max(1) > 0)
+        depth = c["depths"].reshape(b * V, h * w) == 0
+        assert zero.any() and tiny.any() and depth.any(), name
+        for kind, m in (("zero", zero), ("tiny", tiny), ("depth", depth)):
+            for i, p in np.argwhere(m):
+                assert p in pix, (name, kind, p)
+                seen[kind].add((name, int(i)))  # (case, conv item) or (case, scene * V + view)
+        d = Z[f"{name}/d_raw64"]
+        assert np.isfinite(d).all() and np.isfinite(Z[f"{name}/covariances64"]).all()
+        order = Z[f"{name}/pix"].tolist()
+        for i, p in np.argwhere(zero):
+            assert (d[i, 5:9, order.index(p)] == 0).all()
+        for i, p in np.argwhere(tiny):
+            assert (d[i, 5:9, order.index(p)] != 0).any()
+        # the zero depth: a zero covariance at that Gaussian
+        cov = Z[f"{name}/covariances64"]
+        for bv, p in np.argwhere(depth):
+            bi, v = divmod(int(bv), V)
+            if v in (0, V - 1):
+                assert (cov[bi, (0 if v == 0 else h * w) + p] == 0).all()
+    # different scenes or slots: no two kinds share a (case, item)
+    assert len(seen["zero"] & seen["tiny"]) == 0 and all(seen.values())
+
+
+# sha256 over (name, dtype, shape, bytes) of every array of the first eight cases, in name order, as first recorded
+FIRST_CASES_SHA256 = "54c3929f668489c2c13372ba6c5d318d83886af8d87785931ae598347a269104"
+FIRST_CASES = ("b1_v2_13x19_d1", "b1_v2_6x8_d25", "b1_v3_5x6_d25_extremes", "b2_v2_4x4_d9_nan_c2w", "b2_v3_1x7_d16",
+               "b2_v3_4x5_d25_improper", "b2_v3_5x7_d9", "b3_v4_4x5_d4")
+
+
+def test_cases_added_later_leave_the_first_cases_byte_identical():
+    h = hashlib.sha256()
+    keys = sorted(k for k in Z.files if k.split("/")[0] in FIRST_CASES)
+    assert len(keys) == 8 * 19
+    for k in keys:
+        v = Z[k]
+        h.update(k.encode())
+        h.update(str(v.dtype).encode())
+        h.update(str(v.shape).encode())
+        h.update(v.tobytes())
+    assert h.hexdigest() == FIRST_CASES_SHA256
+    assert set(FIRST_CASES) < set(NAMES)
 
 
 def test_oracle_gradient_matches_finite_differences():

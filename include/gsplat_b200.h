@@ -360,7 +360,7 @@ typedef struct GsAdapterConfig {
     const float *c2w;         /* device [V,16] extrinsics, row-major */
     const float *kinv;        /* device [V,9] */
     const float *multiplier;  /* device [V] */
-    const float *sh_rotation; /* device [V,d_sh,d_sh] or NULL */
+    const float *sh_rotation; /* device [V,d_sh,d_sh] or NULL; gs_sh_rotation_blocks on c2w (row_stride 4) writes it */
     const float *sh_mask;     /* device [d_sh] (gaussian_adapter.py:39-46) */
 } GsAdapterConfig;
 
@@ -676,7 +676,9 @@ typedef struct GsGaussianHeadInputs { /* device, contiguous float32 */
     const float *c2w;            /* [batch, views, 4, 4]: refine_sync_abspose.inverse() (:530) */
     const float *intrinsics;     /* [batch, views, 3, 3] normalised (:531) */
     const float *sh_rotation;    /* [batch, 2, d_sh, d_sh] block-diagonal Wigner-D of slot 0 / 1's c2w[:3, :3] after the
-                                    rotation guard (misc/sh_rotation.py:21-34), or NULL = identity */
+                                    rotation guard (misc/sh_rotation.py:21-34), or NULL = identity; gs_sh_rotation_blocks
+                                    on c2w's views 0 and V - 1 (outer batch, inner 2, outer_stride 16 V, inner_stride
+                                    16 (V - 1), row_stride 4) writes it */
     const float *sh_mask;        /* [d_sh] (gaussian_adapter.py:39-46) */
 } GsGaussianHeadInputs;
 
@@ -706,6 +708,35 @@ GS_API int gs_gaussian_head_forward(const GsGaussianHeadConfig *cfg, const GsGau
 GS_API int gs_gaussian_head_backward(const GsGaussianHeadConfig *cfg, const GsGaussianHeadInputs *in,
                                      const GsGaussianHeadOutGrads *gout, const GsGaussianHeadInGrads *gin,
                                      void *stream);
+
+/*
+ * SH rotation (DESIGN.md 5.17): the block-diagonal Wigner-D matrices that GsAdapterConfig::sh_rotation and
+ * GsGaussianHeadInputs::sh_rotation take, as misc/sh_rotation.py:10-36 builds them, for N = outer inner cameras:
+ *   guard   sh_rotation.py:21-22: unless every determinant satisfies |det - 1| <= 1e-8 + 1e-5 (torch.allclose to 1;
+ *           det in fp64 from the fp32 entries; NaN and +-Inf fail), every camera of the call uses the identity
+ *   blocks  per degree l < sqrt(d_sh), D_l(R) with Y_l(R x) = D_l(R) Y_l(x), by pf3plat_b200/sh_rotation.py's
+ *           least-squares fit over 64 fixed unit vectors in fp64, rounded to float32 once
+ * rotations: device float32; matrix (i, s), 0 <= i < outer, 0 <= s < inner, starts at
+ * rotations + i outer_stride + s inner_stride, its rows row_stride floats apart and its columns adjacent, so
+ * contiguous [N, 3, 3] (row_stride 3) and the top-left blocks of a strided [outer, inner, 4, 4] view such as
+ * c2w[:, ::V-1] (row_stride 4) are read in place.  out: device [N, d_sh, d_sh] contiguous, camera i inner + s; every
+ * element is written.  workspace: gs_sh_rotation_workspace_bytes(cfg) bytes of device memory, 4-byte aligned, holding
+ * the guard's flag between the two launches (one stream at a time).  Two launches, no atomics, no host
+ * synchronisation; a camera's matrix depends only on its rotation and the guard.  GS_ERR_INVALID, with nothing
+ * launched, for d_sh not in {1, 4, 9, 16, 25}, outer or inner < 1, N >= 2^31, row_stride not 3 or 4, or a NULL
+ * pointer.
+ */
+typedef struct GsShRotationConfig {
+    int32_t outer, inner;         /* N = outer inner matrices */
+    int64_t outer_stride;         /* floats between matrix (i, s) and (i + 1, s) */
+    int64_t inner_stride;         /* floats between matrix (i, s) and (i, s + 1) */
+    int32_t row_stride;           /* 3 or 4 */
+    int32_t d_sh;                 /* 1, 4, 9, 16 or 25 */
+} GsShRotationConfig;
+
+GS_API int64_t gs_sh_rotation_workspace_bytes(const GsShRotationConfig *cfg); /* -1 for an invalid config */
+GS_API int gs_sh_rotation_blocks(const GsShRotationConfig *cfg, const float *rotations, float *out, void *workspace,
+                                 void *stream);
 
 /*
  * LPIPS-VGG = the `lpips` package's LPIPS(net="vgg", version="0.1"), spatial=False, as PF3plat's LossLpips

@@ -240,6 +240,12 @@ class GsGaussianHeadOutGrads(Structure):
 class GsGaussianHeadInGrads(Structure):
     _fields_ = [(n, c_void_p) for n in ("raw_gaussians", "density_logits", "depths", "c2w", "scratch")]
 
+
+class GsShRotationConfig(Structure):
+    _fields_ = [("outer", c_int32), ("inner", c_int32), ("outer_stride", c_int64), ("inner_stride", c_int64),
+                ("row_stride", c_int32), ("d_sh", c_int32)]
+
+
 SYMBOLS = {
     "gs_abi_version": (c_int, []),
     "gs_last_error": (c_char_p, []),
@@ -316,6 +322,8 @@ SYMBOLS = {
                                          POINTER(GsGaussianHeadOutputs), c_void_p]),
     "gs_gaussian_head_backward": (c_int, [POINTER(GsGaussianHeadConfig), POINTER(GsGaussianHeadInputs),
                                           POINTER(GsGaussianHeadOutGrads), POINTER(GsGaussianHeadInGrads), c_void_p]),
+    "gs_sh_rotation_workspace_bytes": (c_int64, [POINTER(GsShRotationConfig)]),
+    "gs_sh_rotation_blocks": (c_int, [POINTER(GsShRotationConfig), c_void_p, c_void_p, c_void_p, c_void_p]),
 }
 
 

@@ -9,7 +9,7 @@ gaussians_per_pixel = num_surfaces = 1.  Views 0 and V - 1 are selected inside t
 
 Nothing here synchronises the device with the host: K^-1 and the scale multiplier are computed per camera on the device,
 and the reference's SH rotation guard (sh_rotation.py:21, every determinant allclose to 1 or every camera uses the
-identity) is a device flag fed to torch.where.  The backward reduces the per-camera dL/dc2w in a fixed order without
+identity) is a device flag that the Wigner-D kernel reads (csrc/gs_sh_rotation.cu).  The backward reduces the per-camera dL/dc2w in a fixed order without
 atomics, so it is bit-reproducible with or without torch.use_deterministic_algorithms.  Inputs must be float32 CUDA
 tensors; there is no CPU fallback.
 
@@ -26,7 +26,7 @@ from torch import Tensor
 
 from . import _capi
 from .adapter import GaussianAdapterCfg
-from .sh_rotation import sh_rotation_blocks
+from .sh_rotation import guarded_sh_rotation_blocks
 
 _MASKS: dict = {}
 
@@ -66,15 +66,11 @@ def _sh_mask(sh_degree, dev):
 def sh_rotation_for_slots(c2w: Tensor, d_sh: int) -> Tensor | None:
     """[b, 2, d_sh, d_sh] block-diagonal Wigner-D matrices of c2w[:, (0, -1), :3, :3].detach() after the reference's
     all-or-nothing guard (sh_rotation.py:21-22: unless every determinant is allclose to 1, every camera of the call uses
-    the identity; a NaN determinant fails), evaluated on the device.  None for d_sh = 1."""
+    the identity; a NaN determinant fails), built on the device in two launches (csrc/gs_sh_rotation.cu) from the
+    strided view of views 0 and V - 1.  None for d_sh = 1."""
     if d_sh == 1:
         return None
-    c = c2w.detach()
-    rot = torch.stack([c[:, 0, :3, :3], c[:, -1, :3, :3]], 1)  # a tuple index would copy its indices to the device
-    det = torch.det(rot)  # as the reference; batched 3 x 3 determinants make no host read-back
-    ok = torch.isclose(det, torch.ones_like(det)).all()
-    rot = torch.where(ok, rot, torch.eye(3, dtype=rot.dtype, device=rot.device))
-    return sh_rotation_blocks(rot, d_sh).contiguous()
+    return guarded_sh_rotation_blocks(c2w.detach()[:, ::c2w.shape[1] - 1], d_sh)
 
 
 def _structs(raw, logits, depths, c2w, intrinsics, sh_rot, sh_mask, consts):

@@ -11,10 +11,13 @@ it to the coefficients of that degree.  e3nn is a third-party dependency that is
   evaluated at (x_std, y_std, z_std) = (z, x, y); for degree 1 that is the (x, y, z) order and D_1(R) = R.
 
 The fused adapter kernel (pf3plat_b200/adapter.py) takes the block-diagonal matrix as an input, so a caller who has
-e3nn (or any other convention) can always supply its own.
+e3nn (or any other convention) can always supply its own.  `guarded_sh_rotation_blocks` builds that matrix on the
+device, guard included, with the same fit (csrc/gs_sh_rotation.cu); the tensor functions here stay the CPU path and
+the reference it is checked against.
 """
 from __future__ import annotations
 
+import ctypes
 from math import isqrt
 
 import torch
@@ -93,6 +96,54 @@ def sh_rotation_blocks(rotations: torch.Tensor, d_sh: int) -> torch.Tensor:
 def rotations_are_proper(rotations: torch.Tensor) -> bool:
     """The reference's guard (sh_rotation.py:21): every determinant allclose to 1, else ALL rotations -> identity."""
     return bool(torch.allclose(torch.det(rotations), rotations.new_tensor(1)))
+
+
+def guarded_sh_rotation_blocks(rotations: torch.Tensor, d_sh: int) -> torch.Tensor:
+    """The block-diagonal (..., d_sh, d_sh) matrices of sh_rotation_blocks after the reference's all-or-nothing guard
+    (rotate_sh's rotations_are_proper: unless every determinant is allclose to 1, every rotation of the call is the
+    identity), on the device (csrc/gs_sh_rotation.cu): two launches, no host synchronisation, the same least-squares fit
+    in fp64 from the same fit points, rounded to float32 once.
+
+    rotations: float32 CUDA [..., 3, 3], or [..., 4, 4] whose top-left 3 x 3 block is the rotation (c2w itself).  Up to
+    two batch dims are read in place with any strides, so c2w[:, ::V - 1] costs no gather; more are reshaped.  Not
+    differentiable (the reference detaches the rotation, gaussian_adapter.py:81): inputs that require grad are
+    refused."""
+    from . import _capi
+    if not torch.is_tensor(rotations):
+        raise TypeError("guarded_sh_rotation_blocks: rotations must be a tensor")
+    if rotations.device.type != "cuda":
+        raise TypeError(f"guarded_sh_rotation_blocks: rotations must be a CUDA tensor (the tensor route "
+                        f"sh_rotation_blocks is the CPU path), got {rotations.device}")
+    if rotations.dtype != torch.float32:
+        raise TypeError(f"guarded_sh_rotation_blocks: rotations must be float32, got {rotations.dtype}")
+    if rotations.requires_grad:
+        raise ValueError("guarded_sh_rotation_blocks is not differentiable: pass rotations.detach() (the reference "
+                         "detaches the rotation, gaussian_adapter.py:81)")
+    if not isinstance(d_sh, int) or isinstance(d_sh, bool) or d_sh not in (1, 4, 9, 16, 25):
+        raise ValueError(f"guarded_sh_rotation_blocks: d_sh must be 1, 4, 9, 16 or 25, got {d_sh!r}")
+    if rotations.dim() < 2 or tuple(rotations.shape[-2:]) not in ((3, 3), (4, 4)):
+        raise ValueError(f"guarded_sh_rotation_blocks needs [..., 3, 3] or [..., 4, 4] rotations, got "
+                         f"{tuple(rotations.shape)}")
+    batch = rotations.shape[:-2]
+    out = torch.empty(*batch, d_sh, d_sh, dtype=torch.float32, device=rotations.device)
+    if out.numel() == 0:
+        return out
+    r = rotations if len(batch) <= 2 else rotations.reshape(-1, *rotations.shape[-2:])
+    if r.stride(-1) != 1 or r.stride(-2) not in (3, 4):
+        r = r.contiguous()
+    lead = (1,) * (2 - (r.dim() - 2)) + tuple(r.shape[:-2])
+    strides = (0,) * (2 - (r.dim() - 2)) + tuple(r.stride()[:-2])
+    cfg = _capi.GsShRotationConfig(outer=lead[0], inner=lead[1], outer_stride=strides[0], inner_stride=strides[1],
+                                   row_stride=r.stride(-2), d_sh=d_sh)
+    L = _capi.lib()
+    workspace = torch.empty(max(L.gs_sh_rotation_workspace_bytes(ctypes.byref(cfg)), 16), dtype=torch.uint8,
+                            device=r.device)
+    with torch.cuda.device(r.device):
+        stream = ctypes.c_void_p(torch.cuda.current_stream(r.device).cuda_stream)
+        _capi.check(L.gs_sh_rotation_blocks(ctypes.byref(cfg), ctypes.c_void_p(r.data_ptr()),
+                                            ctypes.c_void_p(out.data_ptr()), ctypes.c_void_p(workspace.data_ptr()),
+                                            stream))
+    return out
 
 
 def rotate_sh(sh_coefficients: torch.Tensor, rotations: torch.Tensor) -> torch.Tensor:

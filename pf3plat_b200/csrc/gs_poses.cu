@@ -167,9 +167,28 @@ __device__ void so3_project(const double *a, double *R) {
     for (int c = 1; c < 3; c++)
         if (sig[c] < sig[kmin]) kmin = c;
     for (int c = 0; c < 3; c++)
-        if (c != kmin || sig[c] > 0.0)
+        if (sig[c] > 0.0)
             for (int r = 0; r < 3; r++) W[r][c] /= sig[c];
-    if (!(sig[kmin] > 0.0)) {  // rank 2: complete U by the cross product of its other two columns
+    for (int c = 0; c < 3; c++) {
+        if (c == kmin || sig[c] > 0.0) continue;
+        // rank <= 1: a zero column besides kmin becomes a unit vector orthogonal to the other non-kmin column o: e_c if
+        // o is zero too (so the zero block projects to I, as LAPACK's SVD of zeros gives), else the axis least aligned
+        // with o minus its projection on o
+        const int o = 3 - c - kmin;
+        double e[3] = {0.0, 0.0, 0.0};
+        if (sig[o] > 0.0) {
+            int m = 0;
+            for (int r = 1; r < 3; r++)
+                if (fabs(W[r][o]) < fabs(W[m][o])) m = r;
+            for (int r = 0; r < 3; r++) e[r] = (r == m ? 1.0 : 0.0) - W[m][o] * W[r][o];
+            const double n = sqrt(e[0] * e[0] + e[1] * e[1] + e[2] * e[2]);
+            for (int r = 0; r < 3; r++) e[r] /= n;
+        } else {
+            e[c] = 1.0;
+        }
+        for (int r = 0; r < 3; r++) W[r][c] = e[r];
+    }
+    if (!(sig[kmin] > 0.0)) {  // rank 2 or less: complete U by the cross product of its other two columns
         const int k1 = (kmin + 1) % 3, k2 = (kmin + 2) % 3;
         for (int r = 0; r < 3; r++)
             W[r][kmin] = W[(r + 1) % 3][k1] * W[(r + 2) % 3][k2] - W[(r + 2) % 3][k1] * W[(r + 1) % 3][k2];

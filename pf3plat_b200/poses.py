@@ -14,6 +14,9 @@ Divergences from the reference, none of which PF3plat's training or evaluation r
   as a NaN mass does in the reference.
 - camera_synchronization needs the chain pairs (k, k+1) for every N, because the device decides the fallback.
 - refine_poses on a singular pose returns a non-finite inverse instead of raising.
+- camera_synchronization on a rotation block of rank 1 (reachable only through degenerate pairwise transforms): the
+  reference's answer depends on LAPACK's arbitrary basis of the block's null plane; here it is a proper rotation that
+  agrees with the block on its one singular direction.  The zero block gives I, as in the reference.
 """
 from __future__ import annotations
 

@@ -3,7 +3,8 @@ in float64:
 - `camera_synchronization` (PF3plat's src/flow_util.py, imported unmodified; its module-level `open3d` and
   `pytorch3d.ops` imports are stubbed, nothing here calls them);
 - the refined-pose lines of `EncoderCostVolume.forward` (encoder_costvolume.py:465-473) with the class's own
-  `r6d2mat`, then `.inverse()`, with the autograd gradients of sum(abspose * g_abs + abspose_inv * g_inv);
+  `r6d2mat`, then `.inverse()`, with the autograd gradients of sum(abspose * g_abs + abspose_inv * g_inv) (for the
+  `refine_degenerate_*` cases of sum(abspose * g_abs) alone, with `raises` recording whether `.inverse()` raised);
 - the Plücker lines (:387-392) with projection.py's `sample_image_grid` / `get_world_rays` and the class's own
   `plucker_embedding`.
 The three methods use no instance state; they are taken from the class body with `ast` and run with `self = None`, so
@@ -87,6 +88,55 @@ def sync_case(rng, b, N, trans=0.3, noise=0.03):
             "N": np.int64(N)}
 
 
+def sync_graph(rng, b, N, keys, trans=0.3, noise=0.03):
+    """sync_case on any list of keys, in the given order; a key (i, j) with i > j is the transform i -> j all the same"""
+    Ps = np.zeros((len(keys), b, 4, 4))
+    conf = np.zeros((len(keys), b))
+    for s in range(b):
+        W = [np.eye(4)] + [rigid(rng, 0.3, trans) for _ in range(N - 1)]
+        for q, (i, j) in enumerate(keys):
+            Ps[q, s] = W[j] @ np.linalg.inv(W[i]) @ rigid(rng, noise, noise)
+            c = rng.uniform(0.55, 0.95)
+            conf[q, s] = max(c - 0.5, 0.0) / 0.5 if abs(i - j) > 1 else c
+    return {"keys": np.array(keys, dtype=np.int64), "Ps": Ps.astype(np.float32), "conf": conf.astype(np.float32),
+            "N": np.int64(N)}
+
+
+def chain_keys(N):
+    return [(k, k + 1) for k in range(N - 1)]
+
+
+def shuffled_keys(rng, N, reverse_off_chain):
+    """every pair once, in a shuffled order; off-chain pairs stored as (j, i) where reverse_off_chain draws True"""
+    keys = [(j, i) if j - i > 1 and reverse_off_chain and rng.random() < 0.5 else (i, j)
+            for i, j in itertools.combinations(range(N), 2)]
+    return [keys[q] for q in rng.permutation(len(keys))]
+
+
+# 180-degree rotations about the coordinate axes and the identity: a consistent sign gauge per view
+AXIS_FLIPS = [np.diag(d).astype(np.float64) for d in ((1, 1, 1), (1, -1, -1), (-1, 1, -1), (-1, -1, 1))]
+
+
+def sync_degenerate_rotations(rng, b, N, zero_axes):
+    """pairwise transforms whose rotation parts are D_j D_i Z with D a per-view axis flip and Z the identity with the
+    axes zero_axes[s] zeroed, plus translations: every product along a path is diagonal with entries 0 or +-1, so the
+    rotation part of every synchronised block is diagonal, and zero exactly on the zeroed axes (rank 3 - |zero_axes|)"""
+    keys = list(itertools.combinations(range(N), 2))
+    Ps = np.zeros((len(keys), b, 4, 4))
+    conf = rng.uniform(0.55, 0.95, size=(len(keys), b))
+    for s in range(b):
+        D = [AXIS_FLIPS[0]] + [AXIS_FLIPS[k] for k in rng.integers(0, 4, N - 1)]
+        Z = np.eye(3)
+        for a in zero_axes[s]:
+            Z[a, a] = 0.0
+        for q, (i, j) in enumerate(keys):
+            Ps[q, s] = np.eye(4)
+            Ps[q, s, :3, :3] = D[j] @ D[i] @ Z
+            Ps[q, s, :3, 3] = rng.normal(size=3) * 0.3
+    return {"keys": np.array(keys, dtype=np.int64), "Ps": Ps.astype(np.float32), "conf": conf.astype(np.float32),
+            "N": np.int64(N)}
+
+
 def refine_case(rng, b, v, gamma, trans=1.0):
     R = [rotation(rng.normal(size=3), rng.uniform(0.1, 1.0)) for _ in range(b * v)]
     enc = np.concatenate([np.stack([r[:2].reshape(6) for r in R]).reshape(b, v, 6), rng.normal(size=(b, v, 3)) * trans],
@@ -94,6 +144,17 @@ def refine_case(rng, b, v, gamma, trans=1.0):
     return {"pose_enc": enc.astype(np.float32), "delta": (rng.normal(size=(b, v, 9)) * 0.1).astype(np.float32),
             "gamma": np.float32(gamma), "g_abs": rng.normal(size=(b, v, 4, 4)).astype(np.float32),
             "g_inv": rng.normal(size=(b, v, 4, 4)).astype(np.float32)}
+
+
+def refine_degenerate(rng, b, v, gamma, rot6d):
+    """refine_case with abspose-only cotangents and the 6-d rotation rot6d placed in scene 0 at view 0 and, with a zero
+    delta on its rotation entries (so x is rot6d exactly), in the last scene at the last view"""
+    c = refine_case(rng, b, v, gamma)
+    del c["g_inv"]
+    for s, u in ((0, 0), (b - 1, v - 1)):
+        c["pose_enc"][s, u, :6] = rot6d
+        c["delta"][s, u, :6] = 0.0
+    return c
 
 
 def plucker_case(rng, b, v, h, w):
@@ -134,6 +195,52 @@ def cases():
     out["refine_v5_large_t"] = refine_case(rng, 2, 5, 0.7, trans=500.0)
     out["plucker_8x8"] = plucker_case(rng, 2, 3, 8, 8)
     out["plucker_13x22"] = plucker_case(rng, 1, 2, 13, 22)
+    # cases added later: each draws from its own generator, so the ones above stay byte-identical
+    rng = np.random.default_rng(101)
+    out["sync_sparse_path_n6"] = sync_graph(rng, 2, 6, chain_keys(6))  # only the chain pairs
+    rng = np.random.default_rng(102)
+    out["sync_sparse_ring_n5"] = sync_graph(rng, 2, 5, chain_keys(5) + [(4, 0)])  # one pair stored with i > j
+    rng = np.random.default_rng(103)
+    out["sync_shuffled_n8"] = sync_graph(rng, 2, 8, shuffled_keys(rng, 8, True))
+    rng = np.random.default_rng(104)
+    out["sync_n16"] = sync_graph(rng, 2, 16, list(itertools.combinations(range(16), 2)))
+    rng = np.random.default_rng(105)
+    c = sync_graph(rng, 2, 16, shuffled_keys(rng, 16, False))  # scene 1 has zero mass: 15 chained pairs per view 15
+    c["conf"][:, 1] = 0.0
+    out["sync_chain_n16"] = c
+    rng = np.random.default_rng(106)
+    c = sync_graph(rng, 3, 4, list(itertools.combinations(range(4), 2)))
+    c["conf"][2, 1] = np.nan  # scene 1: a NaN confidence; scene 2: zero mass, which alone would chain the batch
+    c["conf"][:, 2] = 0.0
+    out["sync_nan_and_zero_mass"] = c
+    rng = np.random.default_rng(107)
+    c = sync_graph(rng, 2, 4, chain_keys(4) + [(0, 2), (1, 3)])
+    q13, q23 = 4, 2
+    c["conf"][q23, 1], c["conf"][q13, 1] = 1e-10, -2e-10  # scene 1, view 3: confidences summing below zero
+    out["sync_negative_conf"] = c
+    rng = np.random.default_rng(108)
+    out["sync_rank2"] = sync_degenerate_rotations(rng, 3, 4, [(2,), (1,), (0,)])
+    rng = np.random.default_rng(109)
+    out["sync_rank0"] = sync_degenerate_rotations(rng, 2, 4, [(0, 1, 2)] * 2)
+    degenerate = {
+        "a1_zero": [0.0, 0.0, 0.0, 0.3, -0.8, 0.5],
+        "a1_tiny": [3e-13, -4e-13, 1e-13, 0.3, -0.8, 0.5],            # 0 < |a1| < 1e-12
+        "a2_parallel": [0.0, -0.25, 0.0, 0.0, -0.5, 0.0],             # a2 = 2 a1 on an axis: c is exactly 0
+        "c_above_eps": [0.0, 0.0, 2.0, 1.5e-12, 0.0, 1.0],            # c = (1.5e-12, 0, 0) exactly
+        "c_below_eps": [0.0, 0.0, 2.0, 0.5e-12, -0.5e-12, -0.75],     # c = (5e-13, -5e-13, 0) exactly
+    }
+    for k, (name, rot6d) in enumerate(degenerate.items()):
+        rng = np.random.default_rng(110 + k)
+        out[f"refine_degenerate_{name}"] = refine_degenerate(rng, 2, 3, 0.8, np.float32(rot6d))
+    rng = np.random.default_rng(120)
+    out["refine_degenerate_v1"] = refine_degenerate(rng, 3, 1, 0.8, np.float32([1.0, 0.0, 0.0, 0.0, 1.0, 0.0]))
+    rng = np.random.default_rng(121)
+    out["refine_degenerate_negative_gamma"] = refine_degenerate(rng, 2, 3, -0.7,
+                                                                np.float32([0.0, 0.6, 0.8, 1.0, 0.0, 0.0]))
+    rng = np.random.default_rng(122)
+    c = plucker_case(rng, 1, 2, 1, 37)  # intrinsics in pixel units (rows scaled by w = 37 and h = 1), one pixel high
+    c["intrinsics"][..., 0, :] *= 37.0
+    out["plucker_pixel_units_1x37"] = c
     return out
 
 
@@ -164,9 +271,17 @@ def run_refine(fns, case, dtype):
     pad = torch.zeros_like(Rt[..., 2:3, :])
     pad[..., -1] = 1.0
     A = torch.cat((Rt, pad), dim=-2)
-    Ai = A.inverse()
-    ((A * torch.tensor(case["g_abs"], dtype=dtype)).sum() + (Ai * torch.tensor(case["g_inv"], dtype=dtype)).sum()).backward()
-    return [t.detach().numpy() for t in (A, Ai, enc.grad, delta.grad, gamma.grad)]
+    loss = (A * torch.tensor(case["g_abs"], dtype=dtype)).sum()
+    try:
+        Ai = A.inverse()
+    except Exception:  # a singular abspose: torch.linalg.inv raises torch.linalg.LinAlgError
+        assert "g_inv" not in case
+        Ai = None
+    if "g_inv" in case:  # the cases without g_inv take cotangents on abspose only
+        loss = loss + (Ai * torch.tensor(case["g_inv"], dtype=dtype)).sum()
+    loss.backward()
+    Ai = Ai.detach().numpy() if Ai is not None else np.zeros(0)
+    return [A.detach().numpy(), Ai] + [t.detach().numpy() for t in (enc.grad, delta.grad, gamma.grad)]
 
 
 def run_plucker(proj, fns, case, dtype):
@@ -202,6 +317,8 @@ def main():
                     for k, val in zip(("abspose", "abspose_inv", "d_pose_enc", "d_delta", "d_gamma"),
                                       run_refine(fns, case, dtype)):
                         data[f"{name}/{k}{tag}"] = val
+                    if "g_inv" not in case:
+                        data[f"{name}/raises{tag}"] = np.bool_(data[f"{name}/abspose_inv{tag}"].size == 0)
                 else:
                     data[f"{name}/value{tag}"] = run_plucker(proj, fns, case, dtype)
             finally:

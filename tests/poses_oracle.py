@@ -59,6 +59,8 @@ def build_L(keys, Ps, conf, N, dtype=np.float64):
 
 
 def so3_project(M):
+    """U diag(1, 1, det(U V^T)) V^T.  Unique where M has rank >= 2; for rank <= 1 the SVD's basis is arbitrary, and the
+    tests pin those blocks to the recorded reference (the zero block: I, from LAPACK's SVD of zeros) or to properties"""
     U, _, Vt = np.linalg.svd(M)
     d = np.linalg.det(U @ Vt)
     return (U * np.stack([np.ones_like(d), np.ones_like(d), d], -1)[..., None, :]) @ Vt
@@ -137,10 +139,13 @@ def _normalize_bwd(y, n, g):
 
 
 def refine_backward(pose_enc, delta, gamma, g_abs, g_inv):
-    """gradients of sum(abspose * g_abs + abspose_inv * g_inv) with respect to (pose_enc, delta, gamma)"""
+    """gradients of sum(abspose * g_abs + abspose_inv * g_inv) with respect to (pose_enc, delta, gamma); g_inv None
+    leaves the inverse out (its gradient stays finite where abspose is singular)"""
     A, Ai, f = refine_forward(pose_enc, delta, gamma)
-    AiT = np.swapaxes(Ai, -1, -2)
-    G = np.asarray(g_abs, dtype=np.float64) - AiT @ np.asarray(g_inv, dtype=np.float64) @ AiT
+    G = np.array(g_abs, dtype=np.float64)
+    if g_inv is not None:
+        AiT = np.swapaxes(Ai, -1, -2)
+        G = G - AiT @ np.asarray(g_inv, dtype=np.float64) @ AiT
     gb1, gb2, gb3 = G[..., 0, :3].copy(), G[..., 1, :3].copy(), G[..., 2, :3]
     gx = np.zeros(f["x"].shape)
     gx[..., 6:9] = G[..., :3, 3]

@@ -1,8 +1,9 @@
 """CPU checks of the pose path: the fp64 oracle (tests/poses_oracle.py) and the benchmark's PyTorch restatement of the
 reference (scripts/bench_poses.py) against the reference's own functions recorded in tests/golden/poses.npz
-(make_poses_golden.py); the oracle's refine_poses gradient against central finite differences; the regimes the golden
-cases are meant to reach; the C ABI's struct layouts and argument checks, and the Python entries' refusals (no device)."""
+(make_poses_golden.py), with the cases recorded first held byte-identical; the oracle's refine_poses gradient against
+central finite differences; the regimes the golden cases are meant to reach; the C ABI's struct layouts and argument checks, and the Python entries' refusals (no device)."""
 import ctypes
+import hashlib
 import importlib.util
 import os
 import subprocess
@@ -24,10 +25,20 @@ def load_cases():
 
 CASES = load_cases()
 SYNC = sorted(n for n in CASES if n.startswith("sync"))
-REFINE = sorted(n for n in CASES if n.startswith("refine"))
+# refine cases with cotangents on both outputs; the refine_degenerate_* cases take cotangents on abspose only, and
+# record whether the reference's .inverse() raised
+REFINE = sorted(n for n in CASES if n.startswith("refine") and "g_inv" in CASES[n])
+REFINE_DEGENERATE = sorted(n for n in CASES if n.startswith("refine_degenerate"))
 PLUCKER = sorted(n for n in CASES if n.startswith("plucker"))
 # the reference chains these (N = 2, or the batch fallback)
-CHAINED = {"sync_n2", "sync_all_zero", "sync_one_zero_mass"}
+CHAINED = {"sync_n2", "sync_all_zero", "sync_one_zero_mass", "sync_chain_n16"}
+# synchronised blocks that are not full rank, or masses that are not positive: their regimes are asserted one by one
+DEGENERATE_SYNC = {"sync_rank2", "sync_rank0", "sync_negative_conf"}
+# sha256 over (name, dtype, shape, bytes) of every array of the first sixteen cases, in name order, as first recorded
+FIRST_CASES_SHA256 = "2cff2f0942fcd449bbbc875f312a27787f1adebe26ceb6b13b2cf4b176164c27"
+FIRST_CASES = ("plucker_13x22", "plucker_8x8", "refine_gamma0", "refine_gamma1", "refine_v5_large_t", "sync_all_zero",
+               "sync_large_t", "sync_n2", "sync_n3", "sync_n4", "sync_n5", "sync_n8", "sync_nan_conf",
+               "sync_one_zero_mass", "sync_pnp_fail", "sync_relu_zero_02")
 
 
 def keys_of(case):
@@ -68,6 +79,46 @@ def test_refine_oracle_matches_the_reference_record(name):
     close(gp, c["d_pose_enc64"], 1e-10)
     close(gd, c["d_delta64"], 1e-10)
     close(np.array(gg), c["d_gamma64"], 1e-10)
+
+
+def singular_items(c):
+    """[b, v] True where the refined abspose is exactly singular (a zero 6-d half: b1 or b2 is 0)"""
+    _, _, f = O.refine_forward(c["pose_enc"], c["delta"], c["gamma"])
+    return (f["n1"][..., 0] == 0) | (f["n2"][..., 0] == 0)
+
+
+@pytest.mark.parametrize("name", REFINE_DEGENERATE)
+def test_refine_oracle_matches_the_reference_record_on_degenerate_encodings(name):
+    c = CASES[name]
+    A, Ai, _ = O.refine_forward(c["pose_enc"], c["delta"], c["gamma"])
+    close(A, c["abspose64"], 1e-10)
+    sing = singular_items(c)
+    assert bool(c["raises64"]) == bool(c["raises32"]) == bool(sing.any())
+    if c["raises64"]:  # the reference's .inverse() raises; the oracle's inverse is NaN on the singular items only
+        assert np.isnan(Ai[sing]).all() and np.isfinite(Ai[~sing]).all()
+    else:
+        close(Ai, c["abspose_inv64"], 1e-10)
+    # gradients near the eps clamp are ~1e12 and cancel to ~0 in places: held relative to |ref| + rms ref
+    gp, gd, gg = O.refine_backward(c["pose_enc"], c["delta"], c["gamma"], c["g_abs"], None)
+    for got, ref in ((gp, c["d_pose_enc64"]), (gd, c["d_delta64"]), (np.array(gg), c["d_gamma64"])):
+        assert got.shape == ref.shape and np.isfinite(got).all() and np.isfinite(ref).all()
+        rms = float(np.sqrt((ref ** 2).mean()))
+        assert (np.abs(got - ref) <= 1e-10 * (np.abs(ref) + rms) + 1e-300).all(), name
+
+
+def test_cases_added_later_leave_the_first_cases_byte_identical():
+    z = np.load(GOLDEN)
+    h = hashlib.sha256()
+    keys = sorted(k for k in z.files if k.split("/")[0] in FIRST_CASES)
+    assert len(keys) == 145
+    for k in keys:
+        v = z[k]
+        h.update(k.encode())
+        h.update(str(v.dtype).encode())
+        h.update(str(v.shape).encode())
+        h.update(v.tobytes())
+    assert h.hexdigest() == FIRST_CASES_SHA256
+    assert set(FIRST_CASES) < set(CASES)
 
 
 @pytest.mark.parametrize("name", PLUCKER)
@@ -145,6 +196,8 @@ def test_golden_cases_reach_their_regimes():
         if name in CHAINED:
             assert np.min(mass) == 0  # the batch falls back to chaining
             continue
+        if name in DEGENERATE_SYNC:
+            continue
         assert np.min(mass) > 0 and not bad.any()
         # the polar factor is unique: full rank, and an improper block's smallest singular value is not repeated
         M = blk[..., :3, :3] / mass[..., None, None]
@@ -168,6 +221,79 @@ def test_golden_cases_reach_their_regimes():
     assert not CASES["refine_gamma0"]["d_delta64"].any()  # gamma 0: no gradient reaches delta
     assert np.abs(CASES["refine_v5_large_t"]["pose_enc"][..., 6:]).max() > 100
     assert (CASES["plucker_13x22"]["h"], CASES["plucker_13x22"]["w"]) == (13, 22)
+
+
+def sync_regime(name, l_dtype=np.float64):
+    c = CASES[name]
+    keys, N = keys_of(c), int(c["N"])
+    blk, bad = O.power_column_block(keys, c["Ps"], c["conf"], N, l_dtype=l_dtype)
+    return c, keys, N, blk, bad
+
+
+def test_cases_added_later_reach_their_regimes():
+    # pair graphs: only the chain; the chain and one pair with i > j; every pair in a shuffled order, some reversed
+    c, keys, N, _, _ = sync_regime("sync_sparse_path_n6")
+    assert N == 6 and keys == [(k, k + 1) for k in range(5)] and len(keys) < N * (N - 1) // 2
+    c, keys, N, _, _ = sync_regime("sync_sparse_ring_n5")
+    assert N == 5 and len(keys) == 5 < N * (N - 1) // 2 and (4, 0) in keys
+    for name, N in (("sync_shuffled_n8", 8), ("sync_n16", 16), ("sync_chain_n16", 16)):
+        c, keys, n, _, _ = sync_regime(name)
+        assert n == N and len(keys) == N * (N - 1) // 2 == len({tuple(sorted(k)) for k in keys})
+    for name in ("sync_shuffled_n8", "sync_chain_n16"):  # the chain pairs are not where lexicographic order puts them
+        keys = keys_of(CASES[name])
+        assert keys != sorted(keys)
+        assert [keys.index((k, k + 1)) for k in range(int(CASES[name]["N"]) - 1)] != \
+            [sorted(keys).index((k, k + 1)) for k in range(int(CASES[name]["N"]) - 1)]
+    assert any(i > j for i, j in keys_of(CASES["sync_shuffled_n8"]))
+    # chaining at N = 16: one zero-mass scene, so the healthy scene is chained through 15 pairs too
+    c, keys, N, blk, _ = sync_regime("sync_chain_n16")
+    mass = blk[..., 3, 3]
+    assert (c["conf"][:, 1] == 0).all() and (mass[1] == 0).all() and (mass[0] > 0).all()
+    close(c["value64"], O.camera_chaining(keys, np.asarray(c["Ps"], np.float64), N), 1e-10)
+    # a NaN scene and a zero-mass scene: the NaN mass keeps the batch from chaining; the reference raises
+    c, keys, N, blk, bad = sync_regime("sync_nan_and_zero_mass")
+    assert c["raises64"] and c["raises32"] and list(bad) == [False, True, False]
+    assert (blk[2, :, 3, 3] == 0).all() and (blk[0, :, 3, 3] > 0).all()
+    out = O.camera_synchronization(keys, c["Ps"], c["conf"], N)
+    assert np.isnan(out[1]).all() and np.isfinite(out[[0, 2]]).all()
+    assert not np.allclose(out[0], O.camera_chaining(keys, np.asarray(c["Ps"], np.float64), N)[0])
+    # a negative confidence: one mass ends negative, below the 1e-9 clamp, and the batch is not chained
+    for l_dtype in (np.float64, np.float32):
+        c, keys, N, blk, bad = sync_regime("sync_negative_conf", l_dtype)
+        mass = blk[..., 3, 3]
+        assert (c["conf"] < 0).any() and not bad.any() and mass.min() < 0 and (mass[0] > 0).all()
+    assert np.isfinite(c["value64"]).all() and np.isfinite(c["value32"]).all()
+    # rotation blocks of exact rank 2 (the zeroed axis differs per scene) and exact rank 0, with positive masses
+    for name, rank in (("sync_rank2", 2), ("sync_rank0", 0)):
+        for l_dtype in (np.float64, np.float32):
+            c, keys, N, blk, bad = sync_regime(name, l_dtype)
+            mass = blk[..., 3, 3]
+            assert (mass > 0).all() and not bad.any()
+            sv = np.linalg.svd(blk[..., :3, :3] / mass[..., None, None], compute_uv=False)
+            assert (sv[..., 2] == 0).all(), name  # sigma_min == 0 exactly
+            assert ((sv[..., 1] > 0.1) if rank == 2 else (sv[..., 0] == 0)).all(), name
+    kmin = [np.flatnonzero(np.diag(sync_regime("sync_rank2")[3][s, 1, :3, :3]) == 0) for s in range(3)]
+    assert [list(k) for k in kmin] == [[2], [1], [0]]
+    assert np.array_equal(CASES["sync_rank0"]["value64"][..., :3, :3], np.broadcast_to(np.eye(3), (2, 4, 3, 3)))
+    # degenerate 6-d encodings, each in its own case: at scene 0 view 0 and at the last scene's last view
+    n = {}
+    for name in REFINE_DEGENERATE:
+        c = CASES[name]
+        _, _, f = O.refine_forward(c["pose_enc"], c["delta"], c["gamma"])
+        b, v = c["pose_enc"].shape[:2]
+        n[name] = (f["n1"][..., 0][[0, b - 1], [0, v - 1]], f["n2"][..., 0][[0, b - 1], [0, v - 1]])
+        assert "g_inv" not in c
+    assert (n["refine_degenerate_a1_zero"][0] == 0).all()
+    assert ((n["refine_degenerate_a1_tiny"][0] > 0) & (n["refine_degenerate_a1_tiny"][0] < 1e-12)).all()
+    assert (n["refine_degenerate_a2_parallel"][1] == 0).all()  # a2 = 2 a1: c is exactly 0
+    assert ((n["refine_degenerate_c_above_eps"][1] > 1e-12) & (n["refine_degenerate_c_above_eps"][1] < 2e-12)).all()
+    assert ((n["refine_degenerate_c_below_eps"][1] > 0) & (n["refine_degenerate_c_below_eps"][1] < 1e-12)).all()
+    assert CASES["refine_degenerate_v1"]["pose_enc"].shape[1] == 1
+    assert float(CASES["refine_degenerate_negative_gamma"]["gamma"]) < 0
+    assert [n for n in REFINE_DEGENERATE if CASES[n]["raises64"]] == ["refine_degenerate_a1_zero",
+                                                                      "refine_degenerate_a2_parallel"]
+    c = CASES["plucker_pixel_units_1x37"]
+    assert (int(c["h"]), int(c["w"])) == (1, 37) and (c["intrinsics"][..., 0, 0] > 20).all()
 
 
 @pytest.fixture(scope="module")

@@ -8,20 +8,27 @@ segment.  Pairs [(a, c) for a < c]; segment s = scene * pairs + pair.  Per segme
   dense projection of EVERY pixel of the source view a (as the reference computes it, then gathers):
     X = d_a K_a^-1 [x, y, 1],  Q = T_s [X, 1],  P = Q_xyz / (Q_w + 1e-6),  u = K_c P,  pi = u_xy / (u_z + 1e-6)
   L2_s = sum_n huber_0.01(|pi(p_n) - xy(q_n)|) / 0.01
-  L3_s = conf_s sum_n (w_n / max(sum |w|, 1e-12)) |R_s xyz_a(p_n) + t_s - xyz_c(q_n)|
+  L3_s = conf_s sum_n (w_n / max(sum |w|, eps)) |R_s xyz_a(p_n) + t_s - xyz_c(q_n)|
   loss = weight_3d mean_s L3_s + weight_2d mean_s L2_s.
+The clamp's eps is F.normalize's 1e-12.  The reference trains in float32, where the bound is float32(1e-12) =
+9.99999996e-13 < 1e-12: a segment whose |w| sum is exactly float32(1e-12) passes the clamp in float32 (clamp_min passes
+its gradient at equality) and is clamped in float64.  `EPS_N` reproduces the float64 record, `EPS_N_F32` the float32
+one, which is the truth the kernels follow; `clamp_fragile` names the segments whose sum lies within float32 rounding
+of that bound, where no precision's answer is the reference's.
 Gradients are autograd's through these ops.  The dense projection is kept on purpose: the zero gradient the gather sends
 to an unmatched pixel meets that pixel's projection in the backward, so a non-finite depth there makes dL/ddepth and
 dL/dT_s non-finite exactly as in the reference.  Works on any device and dtype (the tests use float64).
 """
 from __future__ import annotations
 
+import numpy as np
 import torch
 import torch.nn.functional as F
 
 DELTA = 0.01
 EPS_H = 1e-6
 EPS_N = 1e-12
+EPS_N_F32 = float(np.float32(1e-12))
 
 
 def pairs_of(v: int):
@@ -53,7 +60,7 @@ def pack(matches, conf, b, v):
     return sid, id_a, id_c, w, cf
 
 
-def segment_terms(abspose, depth, xyz, K, sid, id_a, id_c, w, cf, h, w_, xy=None):
+def segment_terms(abspose, depth, xyz, K, sid, id_a, id_c, w, cf, h, w_, xy=None, eps=EPS_N):
     """-> (L3 [S], L2 [S]).  abspose [b,v,4,4], depth [b*v,...,h,w], xyz [b,v,3,h,w], K [b,v,3,3]; the packed matches."""
     b, v = abspose.shape[:2]
     pairs = pairs_of(v)
@@ -86,7 +93,7 @@ def segment_terms(abspose, depth, xyz, K, sid, id_a, id_c, w, cf, h, w_, xy=None
     xc = xf[scene, c_n, :, id_c]
     Tn = T.reshape(S, 4, 4)[sid]
     e3 = ((Tn[:, :3, :3] @ xa[:, :, None])[..., 0] + Tn[:, :3, 3] - xc).norm(dim=-1)
-    D = torch.zeros(S, dtype=dt, device=w.device).index_add(0, sid, w.abs()).clamp_min(EPS_N)
+    D = torch.zeros(S, dtype=dt, device=w.device).index_add(0, sid, w.abs()).clamp_min(eps)
     L3 = cf * torch.zeros(S, dtype=dt, device=w.device).index_add(0, sid, w / D[sid] * e3)
     return L3, L2
 
@@ -99,15 +106,47 @@ def pose_loss(abspose, depth, xyz, K, matches, conf, h, w, weight_2d=0.005, weig
     return L3.mean() * weight_3d + L2.mean() * weight_2d
 
 
-def loss_and_grads(abspose, depth, xyz, K, matches, conf, h, w, weight_2d=0.005, weight_3d=0.025, dtype=torch.float64):
+def loss_and_grads(abspose, depth, xyz, K, matches, conf, h, w, weight_2d=0.005, weight_3d=0.025, dtype=torch.float64,
+                   eps=EPS_N):
     """-> dict of the loss and its gradients w.r.t. abspose, depth, xyz, w (packed [M]) and conf ([S]), in `dtype`."""
     b, v = abspose.shape[:2]
     leaf = lambda t: t.detach().to(dtype).clone().requires_grad_(True)
     A, Dp, Xy = leaf(abspose), leaf(depth), leaf(xyz)
     sid, id_a, id_c, wt, cf = pack(matches, conf, b, v)
     wt, cf = leaf(wt), leaf(cf)
-    L3, L2 = segment_terms(A, Dp, Xy, K.detach().to(dtype), sid, id_a, id_c, wt, cf, h, w)
+    L3, L2 = segment_terms(A, Dp, Xy, K.detach().to(dtype), sid, id_a, id_c, wt, cf, h, w, eps=eps)
     loss = L3.mean() * weight_3d + L2.mean() * weight_2d
     gA, gD, gX, gW, gC = torch.autograd.grad(loss, (A, Dp, Xy, wt, cf))
     return {"loss": loss.detach(), "L3": L3.detach(), "L2": L2.detach(), "abspose": gA, "depth": gD, "xyz": gX,
             "w": gW, "conf": gC}
+
+
+def terms_and_grads(abspose, depth, xyz, K, matches, conf, h, w, g3, g2, dtype=torch.float64, eps=EPS_N_F32):
+    """-> dict of L3 [S], L2 [S] and the gradients of sum(g3 L3) + sum(g2 L2) w.r.t. abspose, depth, xyz, w and conf.
+
+    g3 / g2 are per-segment cotangents [S].  None means the term is absent, and an absent term is a zero cotangent
+    through the reference's chain (so 0 x NaN = NaN wherever that chain meets a non-finite value), which is what
+    Losspose itself computes with a weight of 0, and what pf3plat_b200.losses.pose_terms gives when only one of its
+    outputs reaches the loss."""
+    b, v = abspose.shape[:2]
+    leaf = lambda t: t.detach().to(dtype).clone().requires_grad_(True)
+    A, Dp, Xy = leaf(abspose), leaf(depth), leaf(xyz)
+    sid, id_a, id_c, wt, cf = pack(matches, conf, b, v)
+    wt, cf = leaf(wt), leaf(cf)
+    L3, L2 = segment_terms(A, Dp, Xy, K.detach().to(dtype), sid, id_a, id_c, wt, cf, h, w, eps=eps)
+    cot = lambda g, L: torch.zeros_like(L) if g is None else g.detach().to(device=L.device, dtype=dtype)
+    gA, gD, gX, gW, gC = torch.autograd.grad((L3, L2), (A, Dp, Xy, wt, cf), (cot(g3, L3), cot(g2, L2)))
+    return {"L3": L3.detach(), "L2": L2.detach(), "abspose": gA, "depth": gD, "xyz": gX, "w": gW, "conf": gC}
+
+
+def clamp_fragile(matches, b, v, eps=EPS_N_F32):
+    """-> bool [S]: segments whose sum |w| lies within float32 rounding of the clamp's bound (a float32 sum of n terms
+    may be off by (n - 1) 2^-24 of the sum), so that which side of the clamp they fall on depends on the summation.
+    A sum of one weight is exact: a single weight at the bound is not fragile."""
+    sid, _, _, wt, _ = pack(matches, {pr: torch.zeros(b) for pr in pairs_of(v)}, b, v)
+    S = b * len(pairs_of(v))
+    wt = wt.detach().double().cpu()
+    sid = sid.cpu()
+    tot = torch.zeros(S, dtype=torch.float64).index_add(0, sid, wt.abs())
+    n = torch.zeros(S, dtype=torch.float64).index_add(0, sid, torch.ones_like(wt))
+    return (tot - eps).abs() < (n - 1).clamp_min(0) * 2.0 ** -24 * tot

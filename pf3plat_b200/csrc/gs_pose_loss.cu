@@ -159,6 +159,9 @@ __device__ __forceinline__ void block_sums(double (&v)[N], double (*red)[PO_WARP
 
 __device__ __forceinline__ bool index_ok(int64_t p, int64_t hw) { return p >= 0 && p < hw; }
 
+// the normaliser max(sum |w|, 1e-12) as clamp_min computes it: a NaN sum stays NaN (fmax would return the bound)
+__device__ __forceinline__ double clamp_norm(double s) { return s < (double)PO_EPS_N ? (double)PO_EPS_N : s; }
+
 // per segment: sum_n w_n e3_n, sum_n |w_n|, sum_n h2_n, and whether an index is out of range
 __device__ __forceinline__ void segment_sums(const Seg &g, int64_t beg, int64_t end, const int64_t *__restrict__ id_a,
                                              const int64_t *__restrict__ id_c, const float *__restrict__ wts, int v, int h,
@@ -203,7 +206,7 @@ k_pose_loss_fwd(int v, int h, int w, const float *__restrict__ T, const float *_
     segment_sums(g, offsets[s], offsets[s + 1], id_a, id_c, wts, v, h, w, depth, xyz, true, red);
     if (threadIdx.x == 0) {
         const bool bad = red[3][0] != 0.0;
-        const double D = fmax(red[1][0], (double)PO_EPS_N);
+        const double D = clamp_norm(red[1][0]);
         L3[s] = bad ? __int_as_float(0x7fffffff) : (float)((double)g.conf * (red[0][0] / D));
         L2[s] = bad ? __int_as_float(0x7fffffff) : (float)red[2][0];
     }
@@ -230,7 +233,7 @@ k_pose_loss_bwd_match(int v, int h, int w, const float *__restrict__ T, const fl
     __syncthreads();  // red is reused below
     const float nanf_ = __int_as_float(0x7fffffff);
     const float g3 = dL_dL3 ? dL_dL3[s] : 0.f, g2 = dL_dL2 ? dL_dL2[s] : 0.f;
-    const float D = (float)fmax(S_abs, (double)PO_EPS_N);
+    const float D = (float)clamp_norm(S_abs);
     const float c3 = g3 * g.conf;                                    // dL/d(sum_n wn_n e3_n)
     const float dD = S_abs >= (double)PO_EPS_N ? (float)(-(double)c3 * S_we / ((double)D * D)) : 0.f;  // via |w|
     double acc[PO_NRED];

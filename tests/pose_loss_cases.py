@@ -10,6 +10,11 @@ GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "pos
 GOLDEN_CASES = ("v2_b1_16x20", "v3_b2_ragged", "v4_b3_24x24", "v4_b1_zero_weights", "v2_b2_edges",
                 "v3_b1_nan_depth_unmatched", "v3_b1_inf_depth_unmatched", "v3_b2_nonfinite_depth_matched",
                 "v3_b1_nan_xyz_unmatched")
+# cases added later (tests/test_gpu_pose_loss_regimes.py): more views, signed and clamped weights, non-finite weights,
+# confidences, intrinsics and poses, one-pixel-high and one-pixel-wide frames
+NEW_GOLDEN_CASES = ("v5_b2_ragged", "v6_b1_ragged", "v3_b1_signed_weights", "v3_b2_clamp",
+                    "v3_b2_nonfinite_weights_conf", "v3_b2_nonfinite_K", "v3_b2_nonfinite_pose0",
+                    "v3_b2_nonfinite_pose1", "v3_b1_1x37", "v3_b1_37x1")
 GRADS = ("abspose", "depth", "xyz", "w", "conf")
 
 

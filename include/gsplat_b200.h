@@ -286,6 +286,50 @@ GS_API int gs_backward_cam_tanfov(GsContext *ctx, const GsConfig *cfg, const GsI
 
 GS_API void gs_saved_free(GsContext *ctx, GsSaved *saved, void *stream);
 
+/*
+ * Sync-free forward and backward (opt-in, DESIGN.md 5.18): the host never waits for the device, nothing is allocated or
+ * freed and nothing is read back during a call, so a training step around them can be captured in a CUDA graph.  Every
+ * buffer lives in one caller-owned workspace of gs_sync_free_workspace_bytes(cfg, instance_capacity, needs) bytes
+ * (256-byte aligned) that holds at most `instance_capacity` tile instances (the D of GsStats::num_rendered).  The
+ * binning is the exact path's (count, scan, emit, per-tile sort) with every size decision taken on the device.
+ * When a call's D is at most the capacity, colour, depth, alpha and radii are the bytes gs_forward / gs_forward_ex
+ * write, and the gradients those of gs_backward_cam_tanfov (bit for bit under GS_FLAG_DETERMINISTIC).  When it is
+ * larger, nothing is binned: colour, depth and alpha are NaN, the radii are still right, and the backward of that
+ * forward writes NaN into every gradient it produces -- an undersized workspace costs a skipped optimizer step, never a
+ * silently wrong one.  The first 32 bytes of the workspace are uint32 status words: [0] D of the last forward,
+ * [1] its longest tile list, [3] 1 if it exceeded the capacity, [4] 1 if any forward exceeded it since the caller last
+ * zeroed the words, [5] the largest D any forward required since then (words [4] and [5] are only ever raised).
+ * The context's learned shapes, its pool and its pinned read-back word are not touched; GsStats reports
+ * num_rendered = num_visible = max_tile_list = -1 for a sync-free forward.  The GsSaved of a sync-free forward points
+ * into the workspace: gs_saved_free releases only the handle, and the next forward on the same workspace overwrites
+ * what the backward reads.
+ */
+enum {
+    GS_SYNC_FREE_DETERMINISTIC = 1u,  /* room for the GS_FLAG_DETERMINISTIC backward's fixed-point accumulators */
+    GS_SYNC_FREE_CAMERA_GRAD = 2u     /* room for the camera gradient's per-warp partials (cam != NULL) */
+};
+
+typedef struct GsSyncFreeWorkspace {
+    void *base;                 /* device memory, 256-byte aligned */
+    int64_t bytes;              /* size of base */
+    int64_t instance_capacity;  /* 0 .. 2^31-1 tile instances */
+} GsSyncFreeWorkspace;
+
+/* Bytes of a workspace for cfg's P, S, V and frame (the pointers of cfg are not read), `instance_capacity` and the
+ * GS_SYNC_FREE_* bits of `needs`.  GS_ERR_INVALID for a bad configuration or capacity. */
+GS_API int gs_sync_free_workspace_bytes(const GsConfig *cfg, int64_t instance_capacity, uint32_t needs, int64_t *bytes);
+/* gs_forward_ex without a host wait; alpha may be NULL (no alpha plane).  GS_ERR_INVALID, before anything is launched,
+ * when ws is too small for cfg or misaligned. */
+GS_API int gs_forward_sync_free(GsContext *ctx, const GsConfig *cfg, const GsInputs *in, const GsOutputs *out,
+                                const GsAlpha *alpha, const GsSyncFreeWorkspace *ws, GsSaved **saved, void *stream);
+/* gs_backward_cam_tanfov without a host wait, for the GsSaved of gs_forward_sync_free on the same ws.  alpha, cam and
+ * dL_dtanfov may be NULL.  ws needs GS_SYNC_FREE_DETERMINISTIC room under GS_FLAG_DETERMINISTIC and
+ * GS_SYNC_FREE_CAMERA_GRAD room with cam (GS_ERR_INVALID otherwise, before anything is launched). */
+GS_API int gs_backward_sync_free(GsContext *ctx, const GsConfig *cfg, const GsInputs *in, const GsSaved *saved,
+                                 const GsOutGrads *gout, const GsAlpha *alpha, const GsInGrads *gin,
+                                 const GsCameraGrads *cam, float *dL_dtanfov, const GsSyncFreeWorkspace *ws,
+                                 void *stream);
+
 /* GaussianRasterizer.markVisible (unused by PF3plat; kept for surface completeness): present[V,P] = in frustum. */
 GS_API int gs_mark_visible(GsContext *ctx, const GsConfig *cfg, const float *means3D, uint8_t *present, void *stream);
 

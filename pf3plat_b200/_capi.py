@@ -95,6 +95,15 @@ class GsStats(Structure):
                 ("pool_used_bytes", c_int64)]
 
 
+GS_SYNC_FREE_DETERMINISTIC = 1
+GS_SYNC_FREE_CAMERA_GRAD = 2
+
+
+class GsSyncFreeWorkspace(Structure):
+    """A caller-owned workspace of gs_forward_sync_free / gs_backward_sync_free."""
+    _fields_ = [("base", c_void_p), ("bytes", c_int64), ("instance_capacity", c_int64)]
+
+
 # every symbol include/gsplat_b200.h declares: name -> (restype, argtypes)
 class GsAdapterConfig(Structure):
     _fields_ = [("V", c_int32), ("R", c_int32), ("d_sh", c_int32), ("flags", c_uint32),
@@ -271,6 +280,12 @@ SYMBOLS = {
                                        c_void_p]),
     "gs_render_host_ex": (c_int, [c_void_p, POINTER(GsConfig), POINTER(GsInputs), POINTER(GsOutputs), POINTER(GsAlpha),
                                   c_void_p]),
+    "gs_sync_free_workspace_bytes": (c_int, [POINTER(GsConfig), c_int64, c_uint32, POINTER(c_int64)]),
+    "gs_forward_sync_free": (c_int, [c_void_p, POINTER(GsConfig), POINTER(GsInputs), POINTER(GsOutputs), POINTER(GsAlpha),
+                                     POINTER(GsSyncFreeWorkspace), POINTER(c_void_p), c_void_p]),
+    "gs_backward_sync_free": (c_int, [c_void_p, POINTER(GsConfig), POINTER(GsInputs), c_void_p, POINTER(GsOutGrads),
+                                      POINTER(GsAlpha), POINTER(GsInGrads), POINTER(GsCameraGrads), c_void_p,
+                                      POINTER(GsSyncFreeWorkspace), c_void_p]),
     "gs_set_profiling": (c_int, [c_void_p, c_int]),
     "gs_get_stage_ms": (c_int, [c_void_p, POINTER(c_float)]),
     "gs_psnr_scratch_floats": (c_int64, [c_int32, c_int64]),

@@ -95,13 +95,18 @@ k_tile_scan(int nvt, const uint32_t *__restrict__ counters, uint32_t *__restrict
     }
 }
 
+// GATED (sync-free path): nothing is emitted when status[SF_VERDICT] is set, and every exact-capacity store index is
+// checked against `capacity` before the store.
+template <bool GATED = false>
 __global__ void k_emit_buckets(const DevCfg c, const float4 *__restrict__ rec0, const float4 *__restrict__ rec1,
                                const float4 *__restrict__ rec2, const ushort4 *__restrict__ rects,
                                const uint32_t *__restrict__ offsets, const uint32_t sub_cap,
                                const float *__restrict__ strata, const int strata_per_tile,
-                               uint32_t *__restrict__ cursor, uint64_t *__restrict__ bucket) {
+                               uint32_t *__restrict__ cursor, uint64_t *__restrict__ bucket,
+                               const uint32_t *__restrict__ status = nullptr, uint32_t capacity = 0) {
     const size_t g = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (g >= (size_t)c.V * c.P) return;
+    if (GATED && status[SF_VERDICT]) return;
     const ushort4 r = rects[g];
     if (r.z <= r.x || r.w <= r.y) return;
     const uint32_t v = (uint32_t)(g / c.P);
@@ -141,7 +146,10 @@ __global__ void k_emit_buckets(const DevCfg c, const float4 *__restrict__ rec0, 
 #pragma unroll
         for (int k = 0; k < BATCH; k++) {
             if (!ok[k]) continue;
-            if (offsets) bucket[(size_t)offsets[slot[k]] + pos[k]] = key;                     // exact-capacity buckets
+            if (GATED) {
+                const size_t at = (size_t)offsets[slot[k]] + pos[k];
+                if (at < capacity) bucket[at] = key;
+            } else if (offsets) bucket[(size_t)offsets[slot[k]] + pos[k]] = key;              // exact-capacity buckets
             else if (pos[k] < sub_cap) bucket[slot[k] * (size_t)sub_cap + pos[k]] = key;     // fixed-capacity buckets
         }
     }
@@ -384,7 +392,7 @@ int bin_emit_fast(const DevCfg &c, int64_t D, const float4 *rec0, const float4 *
     if (D <= 0) return GS_OK;
     GS_CUDA_OK(cudaMemsetAsync(cursor, 0, bin_counter_bytes(c), st));
     const size_t n = (size_t)c.V * c.P;
-    k_emit_buckets<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(c, rec0, rec1, rec2, rects, offsets, sub_cap, strata,
+    k_emit_buckets<false><<<(unsigned)((n + 255) / 256), 256, 0, st>>>(c, rec0, rec1, rec2, rects, offsets, sub_cap, strata,
                                                                  strata_per_tile, cursor, static_cast<uint64_t *>(scratch));
     GS_CUDA_OK(cudaGetLastError());
     return GS_OK;
@@ -836,6 +844,186 @@ int bin_sort_fallback(const DevCfg &c, int64_t D, const float4 *rec0, const floa
     GS_CUDA_OK(cub::DeviceRadixSort::SortPairs(p, temp_bytes, keys_in, keys_out, vals_in, point_list, (int)D, 0,
                                                tile_bits(c), st));
     k_ranges<<<(unsigned)((D + 255) / 256), 256, 0, st>>>(D, keys_out, ranges);
+    GS_CUDA_OK(cudaGetLastError());
+    return GS_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------------
+// Sync-free binning (DESIGN.md 5.18).  The exact path's count (k_preprocess), k_tile_scan, k_emit_buckets and tile
+// merge sort, with the decisions the host takes there from the read-back words taken on the device instead:
+//   k_capacity_gate  D > capacity: every tile range empty, every tile count zero, the verdict set (emission and the
+//                    sorts then have nothing to do, and the caller's planes become NaN);
+//   size classes     each class of the merge sort is launched over every (view, tile) CTA; a CTA sorts its tile only
+//                    if its list falls in the class, so a short list never pays for an 8192-key sort;
+//   k_tile_sort_long lists longer than BIN_SMEM_CAP, which the exact path hands to the CUB radix fallback: one CTA per
+//                    long (view, tile), an LSD radix sort of the tile's bucket in global memory.
+// No kernel reads or writes past the workspace for any D: stores into the buckets and lists are at offsets below D,
+// and nothing is stored unless D <= capacity.
+// ---------------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256)
+k_capacity_gate(uint32_t nvt, uint32_t capacity, uint32_t *__restrict__ status, const uint32_t *__restrict__ tile_start,
+                uint32_t *__restrict__ tile_n, uint2 *__restrict__ ranges) {
+    const uint32_t D = status[SF_D];
+    const bool over = D > capacity;
+    for (uint32_t vt = blockIdx.x * blockDim.x + threadIdx.x; vt < nvt; vt += gridDim.x * blockDim.x) {
+        const uint32_t start = over ? 0u : tile_start[vt];
+        const uint32_t n = over ? 0u : tile_n[vt];
+        if (over) tile_n[vt] = 0u;
+        ranges[vt] = make_uint2(start, start + n);
+    }
+    if (blockIdx.x == 0 && threadIdx.x == 0) {
+        status[SF_VERDICT] = over ? 1u : 0u;
+        if (over) status[SF_EXCEEDED] = 1u;
+        status[SF_REQUIRED] = max(status[SF_REQUIRED], D);
+    }
+}
+
+// One size class of the tile merge sort: lists of (lo, THREADS * MAX_ITEMS] entries.  Ranges come from the gate.
+template <int THREADS, int MAX_ITEMS>
+__global__ void __launch_bounds__(THREADS)
+k_tile_sort_class(uint32_t lo, const uint32_t *__restrict__ tile_n, const uint32_t *__restrict__ tile_start,
+                  const uint64_t *__restrict__ bucket, uint32_t *__restrict__ point_list) {
+    extern __shared__ __align__(16) unsigned char ts_smem[];
+    const uint32_t vt = blockIdx.x;
+    const uint32_t n = tile_n[vt];
+    if (n <= lo || n > (uint32_t)(THREADS * MAX_ITEMS)) return;
+    const uint32_t off = tile_start[vt];
+    const uint64_t *src = bucket + off;
+    sort_bucket_dispatch<THREADS, MAX_ITEMS>([src](uint32_t i) { return src[i]; }, point_list + off, n, ts_smem);
+}
+
+template <int THREADS, int MAX_ITEMS>
+int launch_tile_sort_class(uint32_t lo, int nvt, const uint32_t *tile_n, const uint32_t *tile_start, const uint64_t *bucket,
+                           uint32_t *point_list, cudaStream_t st) {
+    const size_t smem = tile_sort_smem_bytes<THREADS, MAX_ITEMS>();
+    GS_CUDA_OK(cudaFuncSetAttribute(k_tile_sort_class<THREADS, MAX_ITEMS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    k_tile_sort_class<THREADS, MAX_ITEMS><<<nvt, THREADS, smem, st>>>(lo, tile_n, tile_start, bucket, point_list);
+    GS_CUDA_OK(cudaGetLastError());
+    return GS_OK;
+}
+
+// Lists longer than BIN_SMEM_CAP: a stable LSD radix sort of the 64-bit (depth bits, index) keys, 8-bit digits, between
+// the tile's bucket and its stretch of `tmp`, in chunks of one key per thread.  A key's place in its chunk is its warp's
+// count of the digit before it (match_any) plus the counts of the earlier warps; a pass whose digit is the same for
+// every key would be the identity and is skipped.  The keys are a total order, so the list is the radix fallback's.
+constexpr int LS_THREADS = 1024, LS_WARPS = LS_THREADS / 32, LS_RADIX = 256;
+
+__global__ void __launch_bounds__(LS_THREADS)
+k_tile_sort_long(const uint32_t *__restrict__ tile_n, const uint32_t *__restrict__ tile_start, uint64_t *__restrict__ bucket,
+                 uint64_t *__restrict__ tmp, uint32_t *__restrict__ point_list) {
+    __shared__ uint32_t warp_at[LS_WARPS][LS_RADIX];   // per chunk: warp w's count of digit d, then its first position
+    __shared__ uint32_t hist[LS_RADIX], next[LS_RADIX];
+    __shared__ int s_skip;
+    const uint32_t vt = blockIdx.x;
+    const uint32_t n = tile_n[vt];
+    if (n <= (uint32_t)BIN_SMEM_CAP) return;
+    const uint32_t off = tile_start[vt];
+    const uint32_t tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const uint32_t lt = (1u << lane) - 1u;
+    uint64_t *src = bucket + off, *dst = tmp + off;
+    for (int shift = 0; shift < 64; shift += 8) {
+        for (int d = tid; d < LS_RADIX; d += LS_THREADS) hist[d] = 0u;
+        if (tid == 0) s_skip = 0;
+        __syncthreads();
+        for (uint32_t i = tid; i < n; i += LS_THREADS) atomicAdd(&hist[(uint32_t)(src[i] >> shift) & 255u], 1u);
+        __syncthreads();
+        if (tid < LS_RADIX && hist[tid] == n) s_skip = 1;
+        if (warp == 0) {   // exclusive scan of the histogram: eight digits per lane
+            uint32_t v[8], sum = 0;
+#pragma unroll
+            for (int k = 0; k < 8; k++) {
+                v[k] = hist[lane * 8 + k];
+                sum += v[k];
+            }
+            uint32_t incl = sum;
+#pragma unroll
+            for (int d = 1; d < 32; d <<= 1) {
+                const uint32_t t = __shfl_up_sync(0xffffffffu, incl, d);
+                if ((int)lane >= d) incl += t;
+            }
+            uint32_t run = incl - sum;
+#pragma unroll
+            for (int k = 0; k < 8; k++) {
+                next[lane * 8 + k] = run;
+                run += v[k];
+            }
+        }
+        __syncthreads();
+        const int skip = s_skip;
+        __syncthreads();   // every thread has read it before thread 0 resets it for the next pass
+        if (skip) continue;
+        for (uint32_t c0 = 0; c0 < n; c0 += LS_THREADS) {
+            const uint32_t i = c0 + tid;
+            const bool valid = i < n;
+            const uint64_t key = valid ? src[i] : 0ull;
+            const uint32_t d = valid ? ((uint32_t)(key >> shift) & 255u) : 0xffffffffu;
+            const uint32_t peers = __match_any_sync(0xffffffffu, d);
+            for (int k = tid; k < LS_WARPS * LS_RADIX; k += LS_THREADS) (&warp_at[0][0])[k] = 0u;
+            __syncthreads();
+            if (valid && (peers & lt) == 0) warp_at[warp][d] = __popc(peers);
+            __syncthreads();
+            if (tid < LS_RADIX) {
+                uint32_t run = next[tid];
+                for (int w = 0; w < LS_WARPS; w++) {
+                    const uint32_t cnt = warp_at[w][tid];
+                    warp_at[w][tid] = run;
+                    run += cnt;
+                }
+                next[tid] = run;
+            }
+            __syncthreads();
+            if (valid) dst[warp_at[warp][d] + __popc(peers & lt)] = key;
+            __syncthreads();
+        }
+        uint64_t *t = src;
+        src = dst;
+        dst = t;
+    }
+    __syncthreads();
+    for (uint32_t i = tid; i < n; i += LS_THREADS) point_list[off + i] = (uint32_t)src[i];
+}
+
+// NaN into the arrays of `a` when the verdict is set
+__global__ void __launch_bounds__(256) k_sf_poison(const uint32_t *__restrict__ status, const SfPoison a) {
+    if (!status[SF_VERDICT]) return;
+    const float nan = __int_as_float(0x7fffffff);
+    for (int k = 0; k < a.count; k++)
+        for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < a.n[k]; i += (size_t)gridDim.x * blockDim.x)
+            a.ptr[k][i] = nan;
+}
+
+int bin_sync_free(const DevCfg &c, const SyncFreeBins &b, const float4 *rec0, const float4 *rec1, const float4 *rec2,
+                  cudaStream_t st) {
+    const int nvt = c.V * c.ntiles;
+    const size_t n = (size_t)c.V * c.P;
+    int rc = bin_tile_scan(c, b.tile_counts, b.sub_offsets, b.tile_start, b.tile_n, b.status, st);
+    if (rc != GS_OK) return rc;
+    const unsigned gate_ctas = (unsigned)min((nvt + 255) / 256, 1024);
+    k_capacity_gate<<<gate_ctas, 256, 0, st>>>((uint32_t)nvt, b.capacity, b.status, b.tile_start, b.tile_n, b.ranges);
+    GS_CUDA_OK(cudaGetLastError());
+    if (n > 0) {
+        GS_CUDA_OK(cudaMemsetAsync(b.cursor, 0, bin_counter_bytes(c), st));
+        k_emit_buckets<true><<<(unsigned)((n + 255) / 256), 256, 0, st>>>(c, rec0, rec1, rec2, b.rects, b.sub_offsets, 0,
+                                                                          nullptr, 0, b.cursor, b.bucket, b.status,
+                                                                          b.capacity);
+        GS_CUDA_OK(cudaGetLastError());
+    }
+    // the size classes of bin_sort_fast's ladder: (0, 1024], (1024, 2048], (2048, 4096], (4096, 8192]
+    if ((rc = launch_tile_sort_class<256, 4>(0, nvt, b.tile_n, b.tile_start, b.bucket, b.point_list, st)) != GS_OK) return rc;
+    if ((rc = launch_tile_sort_class<512, 4>(1024, nvt, b.tile_n, b.tile_start, b.bucket, b.point_list, st)) != GS_OK) return rc;
+    if ((rc = launch_tile_sort_class<1024, 4>(2048, nvt, b.tile_n, b.tile_start, b.bucket, b.point_list, st)) != GS_OK) return rc;
+    if ((rc = launch_tile_sort_class<1024, 8>(4096, nvt, b.tile_n, b.tile_start, b.bucket, b.point_list, st)) != GS_OK) return rc;
+    k_tile_sort_long<<<nvt, LS_THREADS, 0, st>>>(b.tile_n, b.tile_start, b.bucket, b.tmp, b.point_list);
+    GS_CUDA_OK(cudaGetLastError());
+    return GS_OK;
+}
+
+int sf_poison_if_exceeded(const uint32_t *status, const SfPoison &arrays, cudaStream_t st) {
+    if (arrays.count == 0) return GS_OK;
+    size_t most = 0;
+    for (int k = 0; k < arrays.count; k++) most = arrays.n[k] > most ? arrays.n[k] : most;
+    const unsigned ctas = (unsigned)(most < (size_t)256 * 512 ? (most + 255) / 256 : 512);
+    k_sf_poison<<<ctas, 256, 0, st>>>(status, arrays);
     GS_CUDA_OK(cudaGetLastError());
     return GS_OK;
 }

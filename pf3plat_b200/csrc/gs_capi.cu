@@ -322,6 +322,10 @@ extern "C" int gs_get_stats(const GsContext *ctx, GsStats *out) {
 extern "C" void gs_saved_free(GsContext *ctx, GsSaved *saved, void *stream) {
     (void)ctx;
     if (!saved) return;
+    if (saved->ws_base) {   // gs_forward_sync_free: the planes belong to the caller's workspace
+        delete saved;
+        return;
+    }
     if (saved->point_list) cudaFreeAsync(saved->point_list, static_cast<cudaStream_t>(stream));
     if (saved->base) cudaFreeAsync(saved->base, static_cast<cudaStream_t>(stream));
     delete saved;
@@ -657,9 +661,16 @@ extern "C" int gs_forward_ex(GsContext *ctx, const GsConfig *cfg, const GsInputs
 }
 
 namespace {
+// What gs_backward_sync_free hands the backward: the workspace's accumulator region (validated to be large enough for
+// this call) and its status words.
+struct SfBwd {
+    unsigned char *scratch;
+    const uint32_t *status;
+};
+
 int backward(GsContext *ctx, const GsConfig *cfg, const GsInputs *in, const GsSaved *saved, const GsOutGrads *gout,
              const float *dL_dalpha, const GsInGrads *gin, void *stream, const GsCameraGrads *cam = nullptr,
-             float *dL_dtanfov = nullptr) {
+             float *dL_dtanfov = nullptr, const SfBwd *sf = nullptr) {
     if (!ctx || !saved || !gout || !gin) return gs_set_error(GS_ERR_INVALID, "null argument");
     int rc = validate(cfg, in);
     if (rc != GS_OK) return rc;
@@ -669,6 +680,8 @@ int backward(GsContext *ctx, const GsConfig *cfg, const GsInputs *in, const GsSa
     DevCfg c = make_dev_cfg(cfg);
     if (saved->P != c.P || saved->V != c.V || saved->S != c.S || saved->H != c.H || saved->W != c.W)
         return gs_set_error(GS_ERR_INVALID, "saved state does not match the configuration");
+    if (!sf && saved->ws_base)
+        return gs_set_error(GS_ERR_INVALID, "the saved state of gs_forward_sync_free needs gs_backward_sync_free");
     c.flags = saved->flags;   // (GS_FLAG_ANTIALIAS included: the backward differentiates what its forward drew)
     if ((rc = validate_antialias(c.flags, cfg->tuning, AA_BWD_KNOBS)) != GS_OK) return rc;
     if (cam && gin->dL_dviewmatrix_z)
@@ -715,13 +728,17 @@ int backward(GsContext *ctx, const GsConfig *cfg, const GsInputs *in, const GsSa
     const size_t acc_bytes = det ? n * (GS_ACC_STRIDE * GS_DET_LIMBS * 8 + 4) : n * GS_ACC_STRIDE * 4;
     const size_t vz_off = align256(acc_bytes);
     const size_t vz_bytes = cam ? camera_grad_scratch_bytes(c) : det ? det_view_z_bytes(c) : 0;
-    rc = ctx->per_gaussian.reserve(vz_bytes ? vz_off + vz_bytes : acc_bytes, 1.0, ctx->pool, st);
-    if (rc != GS_OK) return rc;
-    float *acc = static_cast<float *>(ctx->per_gaussian.p);
+    unsigned char *scratch = sf ? sf->scratch : nullptr;   // (the workspace was checked against this call's needs)
+    if (!sf) {
+        rc = ctx->per_gaussian.reserve(vz_bytes ? vz_off + vz_bytes : acc_bytes, 1.0, ctx->pool, st);
+        if (rc != GS_OK) return rc;
+        scratch = static_cast<unsigned char *>(ctx->per_gaussian.p);
+    }
+    float *acc = reinterpret_cast<float *>(scratch);
     DetAcc da{};
-    if (cam) da.view_z = reinterpret_cast<float *>(static_cast<unsigned char *>(ctx->per_gaussian.p) + vz_off);
+    if (cam) da.view_z = reinterpret_cast<float *>(scratch + vz_off);
     if (det) {
-        unsigned char *base = static_cast<unsigned char *>(ctx->per_gaussian.p);
+        unsigned char *base = scratch;
         da.acc = reinterpret_cast<unsigned long long *>(base);
         da.poison = reinterpret_cast<uint32_t *>(base + n * GS_ACC_STRIDE * GS_DET_LIMBS * 8);
         da.view_z = reinterpret_cast<float *>(base + vz_off);
@@ -729,7 +746,7 @@ int backward(GsContext *ctx, const GsConfig *cfg, const GsInputs *in, const GsSa
     }
     {
         StageTimer t(ctx, GS_STAGE_COMPOSITE_BWD, st);
-        GS_CUDA_OK(cudaMemsetAsync(ctx->per_gaussian.p, 0, acc_bytes, st));
+        GS_CUDA_OK(cudaMemsetAsync(scratch, 0, acc_bytes, st));
         rc = launch_composite_bwd(c, *saved, gout->dL_dcolor, gout->dL_ddepth, acc, st, (cfg->tuning & GS_TUNE_BWD_V1) ? 1 : ((cfg->tuning & GS_TUNE_BWD_OCC4) ? 2 : 0), da,
                                   dL_dalpha);
         if (rc != GS_OK) return rc;
@@ -743,6 +760,28 @@ int backward(GsContext *ctx, const GsConfig *cfg, const GsInputs *in, const GsSa
     ctx->stats.kernel_launches += 2;  // k_composite_bwd, k_preprocess_bwd
     if (det && g.dL_dviewmatrix_z) ctx->stats.kernel_launches += 1;  // k_view_z_finalize
     if (cam) ctx->stats.kernel_launches += 1;                        // k_camera_finalize
+    if (sf) {
+        // the backward of a forward that exceeded its workspace: NaN into every gradient it writes
+        const size_t sp = (size_t)c.S * c.P, vp = (size_t)c.V * c.P, V = (size_t)c.V;
+        SfPoison grads{};
+        grads.add(gin->dL_dmeans3D, sp * 3);
+        grads.add(gin->dL_dmeans2D, vp * 3);
+        grads.add(gin->dL_dshs, sp * c.M * 3);
+        grads.add(gin->dL_dcolors, vp * 3);
+        grads.add(gin->dL_dopacities, sp);
+        grads.add(gin->dL_dscales, sp * 3);
+        grads.add(gin->dL_drotations, sp * 4);
+        grads.add(gin->dL_dcov3D, sp * 6);
+        grads.add(gin->dL_dviewmatrix_z, V * 4);
+        if (cam) {
+            grads.add(cam->dL_dviewmatrix, V * 16);
+            grads.add(cam->dL_dprojmatrix, V * 16);
+            grads.add(cam->dL_dcampos, V * 3);
+            grads.add(dL_dtanfov, V * 2);
+        }
+        if ((rc = sf_poison_if_exceeded(sf->status, grads, st)) != GS_OK) return rc;
+        ctx->stats.kernel_launches += 1;   // k_sf_poison
+    }
     return GS_OK;
 }
 }  // namespace
@@ -770,6 +809,184 @@ extern "C" int gs_backward_cam_tanfov(GsContext *ctx, const GsConfig *cfg, const
                                       const GsCameraGrads *cam, float *dL_dtanfov, void *stream) {
     if (!cam) return gs_set_error(GS_ERR_INVALID, "null camera-gradient request");
     return backward(ctx, cfg, in, saved, gout, alpha ? alpha->dL_dalpha : nullptr, gin, stream, cam, dL_dtanfov);
+}
+
+// ---------------------------------------------------------------------------------------------------------
+// sync-free forward and backward (DESIGN.md 5.18): every buffer in the caller's workspace, every size decision on
+// the device
+// ---------------------------------------------------------------------------------------------------------
+namespace {
+// Workspace layout: status words | saved planes | point_list[capacity] | scratch.  The scratch holds the forward's
+// binning buffers or, once the forward's kernels have run, the backward's accumulators.
+struct SfLayout {
+    GsSaved saved;       // plane pointers; saved.point_list = the workspace's list
+    size_t saved_bytes;  // planes + list
+    SyncFreeBins bins;
+    unsigned char *scratch;
+    size_t bytes;
+};
+
+size_t sf_backward_bytes(const DevCfg &c, uint32_t needs) {
+    const size_t n = (size_t)c.V * c.P;
+    const bool det = (needs & GS_SYNC_FREE_DETERMINISTIC) != 0;
+    const size_t acc = det ? n * (GS_ACC_STRIDE * GS_DET_LIMBS * 8 + 4) : n * GS_ACC_STRIDE * 4;
+    const size_t cam = (needs & GS_SYNC_FREE_CAMERA_GRAD) ? camera_grad_scratch_bytes(c) : 0;
+    const size_t vz = det ? det_view_z_bytes(c) : 0;
+    return align256(acc) + (cam > vz ? cam : vz);
+}
+
+size_t sf_layout(SfLayout *L, const DevCfg &c, size_t capacity, uint32_t needs, unsigned char *base) {
+    size_t off = 0;
+    const size_t n = (size_t)c.V * c.P, nvt = (size_t)c.V * c.ntiles, cap = capacity > 0 ? capacity : 1;
+    auto take = [&](size_t bytes) {
+        unsigned char *p = base ? base + off : nullptr;
+        off += align256(bytes);
+        return p;
+    };
+    *L = SfLayout{};
+    L->bins.capacity = (uint32_t)capacity;
+    L->bins.status = reinterpret_cast<uint32_t *>(take(256));
+    const size_t planes = saved_layout(&L->saved, c, base ? base + off : nullptr);
+    off += planes;
+    L->saved.point_list = reinterpret_cast<uint32_t *>(take(cap * 4));
+    L->bins.point_list = L->saved.point_list;
+    L->bins.ranges = L->saved.ranges;
+    L->saved_bytes = planes + align256(cap * 4);
+    L->scratch = base ? base + off : nullptr;
+    const size_t scratch_off = off;
+    const size_t ctr = bin_counter_bytes(c);
+    L->bins.rects = reinterpret_cast<ushort4 *>(take(n * 8));
+    L->bins.tile_counts = reinterpret_cast<uint32_t *>(take(ctr));
+    L->bins.cursor = reinterpret_cast<uint32_t *>(take(ctr));
+    L->bins.sub_offsets = reinterpret_cast<uint32_t *>(take(nvt * BIN_SUB * 4));
+    L->bins.tile_start = reinterpret_cast<uint32_t *>(take(nvt * 4));
+    L->bins.tile_n = reinterpret_cast<uint32_t *>(take(nvt * 4));
+    L->bins.bucket = reinterpret_cast<uint64_t *>(take(cap * 8));
+    L->bins.tmp = reinterpret_cast<uint64_t *>(take(cap * 8));
+    const size_t bwd_end = scratch_off + sf_backward_bytes(c, needs);
+    L->bytes = off > bwd_end ? off : bwd_end;
+    return L->bytes;
+}
+
+// the dimensions a workspace is sized by (the pointers of cfg are not read)
+int validate_dims(const GsConfig *cfg) {
+    if (!cfg) return gs_set_error(GS_ERR_INVALID, "null config");
+    if (cfg->P < 0 || cfg->S < 1 || cfg->V < 1 || cfg->V % cfg->S != 0)
+        return gs_set_error(GS_ERR_INVALID, "need P >= 0, S >= 1, V >= 1 and V % S == 0");
+    if (cfg->image_height < 1 || cfg->image_width < 1) return gs_set_error(GS_ERR_INVALID, "empty image");
+    if ((int64_t)cfg->P * cfg->V > 0x7fffffffll) return gs_set_error(GS_ERR_OVERFLOW, "P*V exceeds 2^31-1");
+    if ((cfg->image_width + GS_TILE - 1) / GS_TILE > 65535 || (cfg->image_height + GS_TILE - 1) / GS_TILE > 65535)
+        return gs_set_error(GS_ERR_INVALID, "image too large");
+    return GS_OK;
+}
+
+// the workspace against this call: aligned, a capacity the 32-bit lists can index, large enough for cfg and `needs`
+int sf_check(const DevCfg &c, const GsSyncFreeWorkspace *ws, uint32_t needs, SfLayout *L) {
+    if (!ws || !ws->base) return gs_set_error(GS_ERR_INVALID, "null sync-free workspace");
+    if (reinterpret_cast<uintptr_t>(ws->base) & 255u) return gs_set_error(GS_ERR_INVALID, "sync-free workspace not 256-byte aligned");
+    if (ws->instance_capacity < 0 || ws->instance_capacity > 0x7fffffffll)
+        return gs_set_error(GS_ERR_INVALID, "instance_capacity must be in [0, 2^31-1]");
+    if (ws->bytes < 0 || sf_layout(L, c, (size_t)ws->instance_capacity, needs, nullptr) > (size_t)ws->bytes)
+        return gs_set_error(GS_ERR_INVALID, "sync-free workspace smaller than gs_sync_free_workspace_bytes for this "
+                                            "configuration, capacity and backward (GS_SYNC_FREE_*)");
+    sf_layout(L, c, (size_t)ws->instance_capacity, needs, static_cast<unsigned char *>(ws->base));
+    return GS_OK;
+}
+}  // namespace
+
+extern "C" int gs_sync_free_workspace_bytes(const GsConfig *cfg, int64_t instance_capacity, uint32_t needs, int64_t *bytes) {
+    if (!bytes) return gs_set_error(GS_ERR_INVALID, "null bytes");
+    *bytes = -1;
+    int rc = validate_dims(cfg);
+    if (rc != GS_OK) return rc;
+    if (instance_capacity < 0 || instance_capacity > 0x7fffffffll)
+        return gs_set_error(GS_ERR_INVALID, "instance_capacity must be in [0, 2^31-1]");
+    if (needs & ~(uint32_t)(GS_SYNC_FREE_DETERMINISTIC | GS_SYNC_FREE_CAMERA_GRAD))
+        return gs_set_error(GS_ERR_INVALID, "unknown GS_SYNC_FREE_* bit");
+    SfLayout L;
+    *bytes = (int64_t)sf_layout(&L, make_dev_cfg(cfg), (size_t)instance_capacity, needs, nullptr);
+    return GS_OK;
+}
+
+extern "C" int gs_forward_sync_free(GsContext *ctx, const GsConfig *cfg, const GsInputs *in, const GsOutputs *out,
+                                    const GsAlpha *alpha, const GsSyncFreeWorkspace *ws, GsSaved **saved_out,
+                                    void *stream) {
+    if (saved_out) *saved_out = nullptr;
+    if (!ctx || !out) return gs_set_error(GS_ERR_INVALID, "null context/outputs");
+    int rc = validate(cfg, in);
+    if (rc != GS_OK) return rc;
+    if (!out->color || (cfg->P > 0 && !out->radii)) return gs_set_error(GS_ERR_INVALID, "color/radii outputs missing");
+    if ((cfg->flags & GS_FLAG_DEPTH) && !out->depth) return gs_set_error(GS_ERR_INVALID, "GS_FLAG_DEPTH needs out->depth");
+    if (alpha && !alpha->alpha) return gs_set_error(GS_ERR_INVALID, "alpha given without alpha->alpha");
+    if ((rc = validate_depth_mode(cfg)) != GS_OK) return rc;
+    if ((rc = validate_antialias(cfg->flags, cfg->tuning, AA_FWD_KNOBS)) != GS_OK) return rc;
+    const DevCfg c = make_dev_cfg(cfg);
+    SfLayout L;
+    if ((rc = sf_check(c, ws, 0, &L)) != GS_OK) return rc;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    GsSaved *s = new (std::nothrow) GsSaved(L.saved);
+    if (!s) return gs_set_error(GS_ERR_OOM, "host allocation failed");
+    s->base = nullptr;
+    s->ws_base = ws->base;
+    s->bytes = L.saved_bytes;
+    s->D = -1;   // on the device only (status word SF_D)
+    s->P = c.P; s->S = c.S; s->V = c.V; s->H = c.H; s->W = c.W;
+    s->flags = c.flags;
+    s->has_sh = in->shs != nullptr;
+    s->has_scales = in->scales != nullptr;
+    s->depth_mode = cfg->depth_mode;
+    float *alpha_plane = alpha ? alpha->alpha : nullptr;
+    const int pre_variant = ((cfg->tuning & GS_TUNE_PRE_OCC6) ? 1 : 0) | ((cfg->tuning & GS_TUNE_PRE_SH_RAW16) ? 2 : 0);
+    const int composite_variant = (cfg->tuning & GS_TUNE_FWD_WS) ? 2 : 0;
+    const size_t px = (size_t)c.V * c.H * c.W;
+    auto run = [&]() -> int {
+        GS_CUDA_OK(cudaMemsetAsync(L.bins.tile_counts, 0, bin_counter_bytes(c), st));
+        const PreEmit emit{L.bins.tile_counts, nullptr, 0, nullptr, 0};  // sub-bucket = index % BIN_SUB
+        int r = launch_preprocess(c, make_dev_inputs(in), s->rec0, s->rec1, s->rec2, s->meta, out->radii, L.bins.rects,
+                                  emit, st, 0, -1, pre_variant, DepthMode{cfg->depth_mode, cfg->depth_near_far});
+        if (r != GS_OK) return r;
+        if ((r = bin_sync_free(c, L.bins, s->rec0, s->rec1, s->rec2, st)) != GS_OK) return r;
+        if ((r = launch_composite_fwd(c, *s, out->color, out->depth, st, composite_variant, alpha_plane)) != GS_OK) return r;
+        SfPoison planes{};
+        planes.add(out->color, px * 3);
+        if (c.flags & GS_FLAG_DEPTH) planes.add(out->depth, px);
+        planes.add(alpha_plane, px);
+        return sf_poison_if_exceeded(L.bins.status, planes, st);
+    };
+    if ((rc = run()) != GS_OK) {
+        delete s;
+        return rc;
+    }
+    for (bool &valid : ctx->ev_valid) valid = false;
+    // k_preprocess, k_tile_scan, k_capacity_gate, [k_emit_buckets,] 4 size classes + k_tile_sort_long, k_composite_fwd,
+    // k_sf_poison
+    ctx->stats.kernel_launches = (c.P > 0 ? 1 : 0) + 2 + (c.P > 0 ? 1 : 0) + 5 + 1 + 1;
+    ctx->stats.num_rendered = -1;
+    ctx->stats.num_visible = -1;
+    ctx->stats.max_tile_list = -1;
+    ctx->stats.speculative = 0;
+    ctx->stats.saved_bytes = (int64_t)s->bytes;
+    if (saved_out) *saved_out = s;
+    else delete s;
+    return GS_OK;
+}
+
+extern "C" int gs_backward_sync_free(GsContext *ctx, const GsConfig *cfg, const GsInputs *in, const GsSaved *saved,
+                                     const GsOutGrads *gout, const GsAlpha *alpha, const GsInGrads *gin,
+                                     const GsCameraGrads *cam, float *dL_dtanfov, const GsSyncFreeWorkspace *ws,
+                                     void *stream) {
+    if (!ctx || !saved || !gout || !gin) return gs_set_error(GS_ERR_INVALID, "null argument");
+    int rc = validate(cfg, in);
+    if (rc != GS_OK) return rc;
+    if (!ws || !saved->ws_base || saved->ws_base != ws->base)
+        return gs_set_error(GS_ERR_INVALID, "gs_backward_sync_free needs the saved state of gs_forward_sync_free on the same workspace");
+    if (dL_dtanfov && !cam) return gs_set_error(GS_ERR_INVALID, "dL_dtanfov needs the camera gradient (cam)");
+    const uint32_t needs = ((cfg->flags & GS_FLAG_DETERMINISTIC) ? GS_SYNC_FREE_DETERMINISTIC : 0u) |
+                           (cam ? GS_SYNC_FREE_CAMERA_GRAD : 0u);
+    SfLayout L;
+    if ((rc = sf_check(make_dev_cfg(cfg), ws, needs, &L)) != GS_OK) return rc;
+    const SfBwd sf{L.scratch, L.bins.status};
+    return backward(ctx, cfg, in, saved, gout, alpha ? alpha->dL_dalpha : nullptr, gin, stream, cam, dL_dtanfov, &sf);
 }
 
 extern "C" int gs_mark_visible(GsContext *ctx, const GsConfig *cfg, const float *means3D, uint8_t *present,

@@ -57,6 +57,8 @@ struct GsSaved {
     uint32_t flags;
     int has_sh, has_scales;
     int depth_mode;               // GS_DEPTH_* of the forward (its backward chains the same f'(z))
+    const void *ws_base;          // gs_forward_sync_free: the caller's workspace the planes live in (gs_saved_free frees
+                                  // only the handle); NULL: the context's pool
 };
 
 #define GS_CUDA_OK(call)                                                             \
@@ -123,6 +125,42 @@ int bin_sort_spec(const DevCfg &c, uint32_t sub_cap, uint32_t tile_limit, const 
 int bin_sort_fallback(const DevCfg &c, int64_t D, const float4 *rec0, const float4 *rec1, const float4 *rec2,
                       const ushort4 *rects, void *scratch, size_t scratch_bytes, uint32_t *point_list, uint2 *ranges,
                       cudaStream_t st);
+
+// Sync-free binning (gs_forward_sync_free, DESIGN.md 5.18): the exact path's count / scan / emit / per-tile sort with
+// every size decision on the device, inside a caller-owned workspace of fixed instance capacity.  Status words at the
+// workspace's start (uint32): the scan's three result words, this call's verdict, and two words the caller clears.
+enum {
+    SF_D = 0,          // tile instances of the last forward (saturated at 2^32-1)
+    SF_MAX_LIST = 1,   // longest (view, tile) list of the last forward
+    SF_MAX_SUB = 2,    // largest sub-counter of the last forward
+    SF_VERDICT = 3,    // 1: the last forward's D exceeded the capacity (its planes and its backward's gradients are NaN)
+    SF_EXCEEDED = 4,   // 1: some forward since the last clear exceeded the capacity (sticky)
+    SF_REQUIRED = 5,   // largest D any forward since the last clear required (sticky)
+};
+struct SyncFreeBins {
+    uint32_t capacity;                        // instances point_list / bucket / tmp hold
+    uint32_t *status;                         // SF_* words
+    ushort4 *rects;                           // [V*P] candidate tile rectangles (preprocess)
+    uint32_t *tile_counts;                    // padded sub-counters, counted by preprocess
+    uint32_t *cursor;                         // padded sub-cursors of the emission
+    uint32_t *sub_offsets, *tile_start, *tile_n;
+    uint64_t *bucket, *tmp;                   // [capacity] keys; tmp: the long-list sort's second buffer
+    uint32_t *point_list;                     // [capacity]
+    uint2 *ranges;                            // [V*ntiles]
+};
+int bin_sync_free(const DevCfg &c, const SyncFreeBins &b, const float4 *rec0, const float4 *rec1, const float4 *rec2,
+                  cudaStream_t st);
+// NaN into every listed array when status[SF_VERDICT] is set (one launch; nothing is written otherwise)
+struct SfPoison {
+    static constexpr int MAX = 16;
+    float *ptr[MAX];
+    size_t n[MAX];
+    int count;
+    void add(float *p, size_t k) {
+        if (p && k && count < MAX) { ptr[count] = p; n[count] = k; count++; }
+    }
+};
+int sf_poison_if_exceeded(const uint32_t *status, const SfPoison &arrays, cudaStream_t st);
 
 // Deterministic backward (GS_FLAG_DETERMINISTIC, DESIGN.md 5.11): the composite backward adds its terms into exact
 // fixed-point accumulators (gs_det.cuh) instead of the float ones, and the view-matrix gradient is summed in a fixed

@@ -13,6 +13,7 @@ from __future__ import annotations
 
 import atexit
 import ctypes
+import math
 import threading
 from typing import NamedTuple, Optional
 
@@ -20,7 +21,7 @@ import torch
 from torch import nn
 
 from . import _capi
-from ._capi import GsConfig, GsInGrads, GsInputs, GsOutGrads, GsOutputs, GsStats
+from ._capi import GsConfig, GsInGrads, GsInputs, GsOutGrads, GsOutputs, GsStats, GsSyncFreeWorkspace
 
 
 class GaussianRasterizationSettings(NamedTuple):
@@ -117,6 +118,94 @@ def stage_ms(device=None) -> dict:
     arr = (ctypes.c_float * _capi.GS_NUM_STAGES)()
     _capi.check(_capi.lib().gs_get_stage_ms(current_context(device), arr))
     return dict(zip(_capi.STAGE_NAMES, [float(x) for x in arr]))
+
+
+class SyncFreeWorkspace:
+    """Caller-owned memory of the sync-free rasterizer path (gs_forward_sync_free / gs_backward_sync_free, DESIGN.md
+    5.18): one torch-allocated byte buffer that holds the saved state, the tile lists of at most `instance_capacity`
+    tile instances and all scratch of one forward and its backward.  Passing it as `workspace=` to `rasterize_batch` or
+    `render.decoder_forward` selects that path: the host never waits for the device, the library allocates nothing and
+    reads nothing back, so the call can be captured in a CUDA graph.  While a call needs no more instances than the
+    capacity, its outputs are the default path's; past it, colour, depth and alpha are NaN and the backward's gradients
+    too (a NaN-skipping optimizer step then skips the step), and status() reports it.
+
+    The shape (scenes, views, Gaussians per scene, image) is fixed.  `depth`, `alpha` and `camera_grad` say which
+    outputs and gradients calls may ask for, `deterministic` whether their backward may run under
+    torch.use_deterministic_algorithms(True); `buffer` (optional) is a uint8 CUDA tensor, 256-byte aligned, of at least
+    `nbytes` to use instead of a new allocation.  The workspace belongs to one forward at a time: the backward of a
+    forward whose workspace a later forward has reused raises RuntimeError when run eagerly (a CUDA graph replay does
+    not run that check)."""
+
+    def __init__(self, device, scenes: int, views: int, gaussians_per_scene: int, image_shape, instance_capacity: int, *,
+                 depth: bool = False, alpha: bool = False, deterministic: bool = False, camera_grad: bool = False,
+                 buffer: Optional[torch.Tensor] = None):
+        device = torch.device(device)
+        if device.type != "cuda":
+            raise ValueError(f"SyncFreeWorkspace needs a CUDA device, got {device}")
+        if device.index is None:
+            device = torch.device("cuda", torch.cuda.current_device())
+        h, w = (int(x) for x in image_shape)
+        self.dims = (int(scenes), int(views), int(gaussians_per_scene), h, w)
+        self.instance_capacity = int(instance_capacity)
+        self.depth, self.alpha = bool(depth), bool(alpha)
+        self.deterministic, self.camera_grad = bool(deterministic), bool(camera_grad)
+        self.nbytes = sync_free_workspace_bytes(*self.dims, self.instance_capacity, deterministic=self.deterministic,
+                                                camera_grad=self.camera_grad)
+        if buffer is None:
+            buffer = torch.empty(self.nbytes, dtype=torch.uint8, device=device)
+        elif buffer.device != device or buffer.dtype != torch.uint8 or not buffer.is_contiguous():
+            raise ValueError(f"buffer must be a contiguous uint8 tensor on {device}")
+        elif buffer.numel() < self.nbytes or buffer.data_ptr() % 256:
+            raise ValueError(f"buffer must hold {self.nbytes} bytes at a 256-byte aligned address")
+        self.buffer = buffer
+        self.device = device
+        self.generation = 0   # forwards run on it (the eager reuse check of the backward)
+        self._ws = GsSyncFreeWorkspace(buffer.data_ptr(), buffer.numel(), self.instance_capacity)
+        self.clear_status()
+
+    def status(self) -> tuple:
+        """(required_instances, exceeded): the most tile instances any forward since the last clear_status() needed, and
+        whether any of them exceeded the capacity.  Synchronises with the device."""
+        words = self.buffer[:32].view(torch.int32).cpu().tolist()
+        return words[5] & 0xffffffff, bool(words[4])
+
+    def clear_status(self) -> None:
+        """Resets the status words (stream-ordered; graph-capturable)."""
+        self.buffer[:32].zero_()
+
+    def _check(self, dev, S, V, P, H, W, with_depth, with_alpha, camera) -> None:
+        if dev != self.device:
+            raise ValueError(f"the workspace is on {self.device}, the inputs on {dev}")
+        if (S, V, P, H, W) != self.dims:
+            raise ValueError(f"the workspace was sized for (scenes, views, gaussians, height, width) = {self.dims}, "
+                             f"the call has {(S, V, P, H, W)}")
+        for wanted, have, name in ((with_depth, self.depth, "depth"), (with_alpha, self.alpha, "alpha"),
+                                   (camera, self.camera_grad, "camera_grad")):
+            if wanted and not have:
+                raise ValueError(f"the call needs a workspace created with {name}=True")
+
+
+def sync_free_workspace_bytes(scenes: int, views: int, gaussians_per_scene: int, height: int, width: int,
+                              instance_capacity: int, *, deterministic: bool = False, camera_grad: bool = False) -> int:
+    """Bytes of a SyncFreeWorkspace (gs_sync_free_workspace_bytes); ValueError for a bad shape or capacity."""
+    cfg = GsConfig()
+    cfg.P, cfg.S, cfg.V, cfg.image_height, cfg.image_width = (int(gaussians_per_scene), int(scenes), int(views),
+                                                              int(height), int(width))
+    needs = ((_capi.GS_SYNC_FREE_DETERMINISTIC if deterministic else 0) |
+             (_capi.GS_SYNC_FREE_CAMERA_GRAD if camera_grad else 0))
+    out = ctypes.c_int64()
+    _capi.check(_capi.lib().gs_sync_free_workspace_bytes(ctypes.byref(cfg), int(instance_capacity), needs,
+                                                         ctypes.byref(out)))
+    return out.value
+
+
+def sync_free_capacity(margin: float = 1.5, device=None) -> int:
+    """An instance capacity for a SyncFreeWorkspace: the tile instances of the last default forward on this device and
+    stream (last_stats()["num_rendered"]) times `margin`."""
+    n = last_stats(device)["num_rendered"]
+    if n < 0:
+        raise RuntimeError("the last forward on this context did not report its tile instances (a sync-free call)")
+    return int(math.ceil(n * float(margin)))
 
 
 class _SavedHandle:
@@ -317,7 +406,7 @@ class _RasterizeBatch(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, means3D, means2D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp, viewmatrix,
-                projmatrix, campos, tanfov, bs: BatchSettings):
+                projmatrix, campos, tanfov, bs: BatchSettings, workspace: Optional[SyncFreeWorkspace] = None):
         # an output the loss does not use arrives in backward as None instead of a zero tensor: a colour-only loss
         # then gives the view matrices no gradient at all (and the kernels read no depth gradient: the same sums)
         ctx.set_materialize_grads(False)
@@ -353,8 +442,16 @@ class _RasterizeBatch(torch.autograd.Function):
                                             (means3D, means2D, shs, colors_precomp, opacities, scales, rotations,
                                              cov3D_precomp))
             saved = ctypes.c_void_p()
+            if workspace is not None:
+                workspace._check(dev, S, V, P, H, W, bs.with_depth, bs.with_alpha, want_cam)
             with _context_lock(dev, stream_ptr):
-                if alpha is not None:
+                if workspace is not None:
+                    workspace.generation += 1
+                    rc = _capi.lib().gs_forward_sync_free(
+                        gctx, ctypes.byref(cfg), ctypes.byref(gin), ctypes.byref(gout),
+                        ctypes.byref(_capi.GsAlpha(_ptr(alpha), None)) if alpha is not None else None,
+                        ctypes.byref(workspace._ws), ctypes.byref(saved) if needs_grad else None, stream_ptr)
+                elif alpha is not None:
                     rc = _capi.lib().gs_forward_ex(gctx, ctypes.byref(cfg), ctypes.byref(gin), ctypes.byref(gout),
                                                    ctypes.byref(_capi.GsAlpha(_ptr(alpha), None)),
                                                    ctypes.byref(saved) if needs_grad else None, stream_ptr)
@@ -365,6 +462,8 @@ class _RasterizeBatch(torch.autograd.Function):
         if needs_grad:
             ctx.handle = _SavedHandle(gctx, saved, stream_ptr, dev)
             ctx.bs = bs
+            ctx.workspace = workspace
+            ctx.ws_generation = None if workspace is None else workspace.generation
             ctx.ins = ins            # contiguous fp32 inputs the backward kernels re-read
             # `ins` aliases the caller's tensors when they already are fp32-contiguous; autograd's own version check is
             # bypassed for them, so do it by hand: an in-place update between forward and backward must raise, as it
@@ -391,6 +490,10 @@ class _RasterizeBatch(torch.autograd.Function):
                                    f"operation: {name} is at version {t._version}; expected version {version} instead")
         dev = ins["means3D"].device
         bs = ctx.bs
+        ws = ctx.workspace
+        if ws is not None and ws.generation != ctx.ws_generation:
+            raise RuntimeError("the sync-free workspace of this forward has been reused by a later forward: its saved "
+                               "state is gone (run the backward before the next forward on the workspace)")
         grad_depth = grad_extra[0] if bs.with_depth else None
         # an alpha the loss does not read arrives as None: the call is then gs_backward's, kernels included
         grad_alpha = grad_extra[-1] if bs.with_alpha else None
@@ -420,8 +523,17 @@ class _RasterizeBatch(torch.autograd.Function):
             ig = GsInGrads(**{k: _ptr(t) for k, t in g.items()})
             # (dL/dtanfov only when tanfov requires grad: the other three are the same bytes with or without it)
             gcam = [e(V, 16), e(V, 16), e(V, 3), e(V, 2) if ctx.cam[3][3] else None] if ctx.cam is not None else None
+            if ws is not None and cfg.flags & _capi.GS_FLAG_DETERMINISTIC and not ws.deterministic:
+                raise ValueError("a deterministic backward needs a workspace created with deterministic=True")
             with _context_lock(dev, stream_ptr):
-                if gcam is not None:
+                if ws is not None:
+                    galpha = _f32c(grad_alpha)
+                    rc = _capi.lib().gs_backward_sync_free(
+                        gctx, ctypes.byref(cfg), ctypes.byref(gin), ctx.handle.ptr, ctypes.byref(og),
+                        ctypes.byref(_capi.GsAlpha(None, _ptr(galpha))), ctypes.byref(ig),
+                        ctypes.byref(_capi.GsCameraGrads(*[_ptr(t) for t in gcam[:3]])) if gcam is not None else None,
+                        _ptr(gcam[3]) if gcam is not None else None, ctypes.byref(ws._ws), stream_ptr)
+                elif gcam is not None:
                     galpha = _f32c(grad_alpha)
                     rc = _capi.lib().gs_backward_cam_tanfov(
                         gctx, ctypes.byref(cfg), ctypes.byref(gin), ctx.handle.ptr, ctypes.byref(og),
@@ -447,22 +559,23 @@ class _RasterizeBatch(torch.autograd.Function):
                 shape, dtype = ctx.view_z
                 gview = gview.reshape(shape).to(dtype)
         return (g["dL_dmeans3D"], g["dL_dmeans2D"], g["dL_dshs"], g["dL_dcolors"], g["dL_dopacities"],
-                g["dL_dscales"], g["dL_drotations"], g["dL_dcov3D"], gview, gproj, gcampos, gtan, None)
+                g["dL_dscales"], g["dL_drotations"], g["dL_dcov3D"], gview, gproj, gcampos, gtan, None, None)
 
 
 def rasterize_batch(bs: BatchSettings, means3D, opacities, shs=None, colors_precomp=None, scales=None,
-                    rotations=None, cov3D_precomp=None, means2D=None):
+                    rotations=None, cov3D_precomp=None, means2D=None, *, workspace: Optional[SyncFreeWorkspace] = None):
     """Batched operator.  Shapes: means3D (S,P,3); opacities (S,P) or (S,P,1); shs (S,P,M,3); colors_precomp
     (V,P,3); scales (S,P,3); rotations (S,P,4); cov3D_precomp (S,P,6); means2D (V,P,3) (gradient sink only).
     Returns (color (V,3,H,W), radii (V,P)[, depth (V,H,W)][, alpha (V,H,W)]).  With bs.with_depth, a bs.viewmatrix that
     requires grad gets dL/ddepth's gradient in its z column (see _RasterizeBatch); bs.with_alpha appends the accumulated
     opacity 1 - T_final.  With bs.camera_gradients, bs.viewmatrix, bs.projmatrix, bs.campos and bs.tanfov that require
-    grad get the full camera gradient instead."""
+    grad get the full camera gradient instead.  `workspace` (a SyncFreeWorkspace of this call's shape) selects the
+    sync-free path: no host wait, no allocation by the library, graph-capturable; None = the default path."""
     _check_exclusive(shs, colors_precomp, scales, rotations, cov3D_precomp)
     # means2D exists in the reference op only as a sink for the screen-space gradient (cuda_splatting.py:93-97); the
     # batched entry neither allocates nor fills it unless the caller passes one
     return _RasterizeBatch.apply(means3D, means2D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp,
-                                 bs.viewmatrix, bs.projmatrix, bs.campos, bs.tanfov, bs)
+                                 bs.viewmatrix, bs.projmatrix, bs.campos, bs.tanfov, bs, workspace)
 
 
 def _check_exclusive(shs, colors_precomp, scales, rotations, cov3D_precomp):

@@ -34,7 +34,7 @@ def render_views(extrinsics, intrinsics, near, far, image_shape, background_colo
                  gaussian_covariances, gaussian_sh_coefficients, gaussian_opacities, scale_invariant: bool = True,
                  use_sh: bool = True, with_depth: bool = False, sh_layout: str = "g_xyz_n",
                  sh_eval_max_degree: Optional[int] = None, depth_mode: str = "depth", with_alpha: bool = False,
-                 antialiasing: Optional[bool] = None, camera_gradients: Optional[bool] = None):
+                 antialiasing: Optional[bool] = None, camera_gradients: Optional[bool] = None, workspace=None):
     """extrinsics (B,4,4) c2w, intrinsics (B,3,3), near/far (B,), background (B,3); Gaussians are per SCENE and NOT
     repeated per view: means (S,G,3), covariances (S,G,3,3) or (S,G,6), sh (S,G,3,d_sh) [or (S,G,d_sh,3) with
     sh_layout="g_n_xyz"], opacities (S,G); B % S == 0 and view b shows scene b // (B//S).
@@ -49,7 +49,8 @@ def render_views(extrinsics, intrinsics, near, far, image_shape, background_colo
     camera_gradients: extrinsics and intrinsics that require grad get the full gradient of every output (colour, depth,
     alpha, the anti-aliasing factor) through render_cuda's own camera glue (make_view_batch; the intrinsics through the
     fov, into tanfov and P); None = the process-wide setting (rasterizer.set_camera_gradients, default off: only the
-    depth channel reaches the extrinsics, and the intrinsics get none)."""
+    depth channel reaches the extrinsics, and the intrinsics get none).
+    workspace: a rasterizer.SyncFreeWorkspace of this call's shape selects the sync-free path (rasterize_batch)."""
     assert use_sh or gaussian_sh_coefficients.shape[-1 if sh_layout == "g_xyz_n" else -2] == 1
     h, w = image_shape
     if camera_gradients is None:
@@ -74,11 +75,12 @@ def render_views(extrinsics, intrinsics, near, far, image_shape, background_colo
     B = extrinsics.shape[0]
     S = gaussian_means.shape[0]
     if use_sh:
-        out = rasterize_batch(bs, gaussian_means, gaussian_opacities, shs=shs, cov3D_precomp=cov6)
+        out = rasterize_batch(bs, gaussian_means, gaussian_opacities, shs=shs, cov3D_precomp=cov6, workspace=workspace)
     else:
         colors = shs[..., 0, :]                                  # (S,G,3)
         colors = colors.repeat_interleave(B // S, dim=0) if S != B else colors
-        out = rasterize_batch(bs, gaussian_means, gaussian_opacities, colors_precomp=colors, cov3D_precomp=cov6)
+        out = rasterize_batch(bs, gaussian_means, gaussian_opacities, colors_precomp=colors, cov3D_precomp=cov6,
+                              workspace=workspace)
     if with_alpha:
         return (out[0], out[2], out[3]) if with_depth else (out[0], out[2])
     if with_depth:
@@ -97,7 +99,7 @@ def render_cuda(extrinsics, intrinsics, near, far, image_shape, background_color
 def decoder_forward(means, covariances, harmonics, opacities, extrinsics, intrinsics, near, far, image_shape,
                     background_color, depth_mode: Optional[str] = None, sh_eval_max_degree: Optional[int] = None,
                     return_alpha: bool = False, antialiasing: Optional[bool] = None,
-                    camera_gradients: Optional[bool] = None):
+                    camera_gradients: Optional[bool] = None, workspace=None):
     """`DecoderSplattingCUDA.forward` (decoder_splatting_cuda.py:35-67) without the v-fold repeat: Gaussians
     (b,g,...), cameras (b,v,...).  Returns (color (b,v,3,h,w), depth (b,v,h,w) or None).  Every depth_mode of the
     reference ("depth", "disparity", "relative_disparity", "log") is composited in the same pass as the colour.
@@ -116,14 +118,16 @@ def decoder_forward(means, covariances, harmonics, opacities, extrinsics, intrin
     camera_gradients (None = rasterizer.get_camera_gradients(), default off): the extrinsics get the full gradient of
     every output instead -- colour, depth (the z-column route above is then part of it, not added again), alpha and
     the anti-aliasing factor -- for photometric pose training and test-time pose refinement; intrinsics that require
-    grad get theirs too, in all nine entries (focal refinement, calibration-free use)."""
+    grad get theirs too, in all nine entries (focal refinement, calibration-free use).
+    workspace: a rasterizer.SyncFreeWorkspace for (b, b*v, g, image_shape) selects the sync-free path: the call never
+    makes the host wait, so decoder, loss and backward can be captured in one CUDA graph (INTEGRATION.md)."""
     b, v = extrinsics.shape[:2]
     flat = lambda t: t.reshape(b * v, *t.shape[2:])
     bg = background_color.reshape(1, 3).expand(b * v, 3)
     out = render_views(flat(extrinsics), flat(intrinsics), flat(near), flat(far), image_shape, bg, means,
                        covariances, harmonics, opacities, with_depth=depth_mode is not None,
                        sh_eval_max_degree=sh_eval_max_degree, depth_mode=depth_mode or "depth", with_alpha=return_alpha,
-                       antialiasing=antialiasing, camera_gradients=camera_gradients)
+                       antialiasing=antialiasing, camera_gradients=camera_gradients, workspace=workspace)
     alpha = None
     if return_alpha:
         *out, alpha = out

@@ -783,6 +783,54 @@ GS_API int gs_sh_rotation_blocks(const GsShRotationConfig *cfg, const float *rot
                                  void *stream);
 
 /*
+ * Optimizer step = PF3plat's ModelWrapper.optimizer_step after its closure (src/model/model_wrapper.py:224-241): skip
+ * the step when any gradient holds a NaN, else clip_grad_norm_(max_norm) as Lightning's gradient_clip_val does and
+ * torch.optim.Adam's update (one param group, no weight decay, no amsgrad), then zero_grad(set_to_none=False).
+ * Three launches for any number of tensors, no host synchronisation, no float atomics (bit-reproducible):
+ *   1. per chunk, the sum of squares of its gradient in fp64 and whether it holds a NaN (x != x; Inf does not skip);
+ *   2. one CTA: the fixed-order reduction to the skip verdict and the clip coefficient
+ *      coef = min(max_norm * (1 / (||g||_2 + 1e-6)), 1) in fp32, ||g||_2 the fp64 sum's root rounded once (inf past
+ *      FLT_MAX, where torch's fp32 squares overflow); unless skipped, every tensor's step count + 1 and its
+ *      bias corrections in fp64 from it, rounded to fp32 as torch rounds its scalars; on a skip, *skipped += 1;
+ *   3. per chunk, unless skipped: g = coef g, exp_avg = lerp(exp_avg, g, 1 - beta1),
+ *      exp_avg_sq = exp_avg_sq beta2 + (1 - beta2) g^2, param += -lr / bc1 * exp_avg / (sqrt(exp_avg_sq) / sqrt(bc2)
+ *      + eps), as torch's non-capturable foreach Adam; the gradient is zeroed (zero_grads != 0) whether or not skipped.
+ * The chunk table lists every tensor that has a gradient.  Each chunk covers elements [begin, begin + count) of its
+ * tensor, count <= GS_ADAM_CHUNK; the chunks of one tensor are consecutive and a tensor with no element has one chunk
+ * of count 0 (its step still advances).  tensor < cfg->tensors indexes steps (float32, torch's dtype for the step); a
+ * tensor index that never appears keeps its step.  Pointers need only 4-byte alignment: chunks whose four arrays are
+ * 16-byte aligned run on 16-byte accesses, the others element by element.
+ * lr: device float32 (one value, read by the device).  skipped: device int32, incremented per skipped step.
+ * scratch: gs_adam_scratch_bytes(cfg) bytes, 256-byte aligned, for one stream at a time.  GS_ERR_INVALID, with nothing
+ * launched, for tensors or chunks < 1, beta outside [0, 1), eps < 0 or not finite, a NaN or infinite max_norm, or a
+ * NULL pointer.
+ */
+#define GS_ADAM_CHUNK 16384   /* most elements per chunk */
+
+typedef struct GsAdamChunk {
+    float *param;        /* the tensor's first element (not the chunk's) */
+    float *grad;
+    float *exp_avg;
+    float *exp_avg_sq;
+    int64_t begin;       /* the chunk's first element within its tensor */
+    int32_t count;       /* 0 .. GS_ADAM_CHUNK */
+    int32_t tensor;      /* 0 .. tensors - 1 */
+} GsAdamChunk;
+
+typedef struct GsAdamConfig {
+    int32_t tensors;     /* entries of steps */
+    int32_t chunks;      /* entries of the chunk table */
+    double beta1, beta2, eps;
+    double max_norm;     /* < 0: no clip (Lightning's gradient_clip_val=None) */
+    int32_t zero_grads;  /* 0 or 1 */
+    int32_t reserved_;
+} GsAdamConfig;
+
+GS_API int64_t gs_adam_scratch_bytes(const GsAdamConfig *cfg); /* -1 for an invalid config */
+GS_API int gs_adam_step(const GsAdamConfig *cfg, const GsAdamChunk *chunks, float *steps, const float *lr,
+                        int32_t *skipped, void *scratch, void *stream);
+
+/*
  * LPIPS-VGG = the `lpips` package's LPIPS(net="vgg", version="0.1"), spatial=False, as PF3plat's LossLpips
  * (src/loss/loss_lpips.py:55-59) and compute_lpips (src/evaluation/metrics.py:27-33) call it; forward and input
  * gradients (the weights are constants).  The weights are an input:

@@ -8,7 +8,7 @@ from __future__ import annotations
 
 import ctypes
 import os
-from ctypes import POINTER, Structure, c_char_p, c_float, c_int, c_int8, c_int32, c_int64, c_uint32, c_void_p
+from ctypes import POINTER, Structure, c_char_p, c_double, c_float, c_int, c_int8, c_int32, c_int64, c_uint32, c_void_p
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "csrc", "libgsplat_b200.so")
@@ -255,6 +255,19 @@ class GsShRotationConfig(Structure):
                 ("row_stride", c_int32), ("d_sh", c_int32)]
 
 
+GS_ADAM_CHUNK = 16384
+
+
+class GsAdamChunk(Structure):
+    _fields_ = [(n, c_void_p) for n in ("param", "grad", "exp_avg", "exp_avg_sq")] + [
+        ("begin", c_int64), ("count", c_int32), ("tensor", c_int32)]
+
+
+class GsAdamConfig(Structure):
+    _fields_ = [("tensors", c_int32), ("chunks", c_int32), ("beta1", c_double), ("beta2", c_double), ("eps", c_double),
+                ("max_norm", c_double), ("zero_grads", c_int32), ("reserved_", c_int32)]
+
+
 SYMBOLS = {
     "gs_abi_version": (c_int, []),
     "gs_last_error": (c_char_p, []),
@@ -339,6 +352,8 @@ SYMBOLS = {
                                           POINTER(GsGaussianHeadOutGrads), POINTER(GsGaussianHeadInGrads), c_void_p]),
     "gs_sh_rotation_workspace_bytes": (c_int64, [POINTER(GsShRotationConfig)]),
     "gs_sh_rotation_blocks": (c_int, [POINTER(GsShRotationConfig), c_void_p, c_void_p, c_void_p, c_void_p]),
+    "gs_adam_scratch_bytes": (c_int64, [POINTER(GsAdamConfig)]),
+    "gs_adam_step": (c_int, [POINTER(GsAdamConfig), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
 }
 
 

@@ -7,7 +7,7 @@ ARCH="-gencode arch=compute_90a,code=sm_90a"
 FLAGS="$ARCH -O3 -lineinfo -std=c++17 -Xcompiler -fPIC -Xcompiler -fvisibility=hidden --expt-relaxed-constexpr"
 OBJS=""
 PIDS=""
-for f in gs_capi gs_preprocess gs_binning gs_composite_fwd gs_composite_bwd gs_preprocess_bwd gs_metrics gs_losses gs_pose_loss gs_lpips gs_adapter gs_cameras gs_costvolume gs_poses gs_encoder_depth gs_gaussian_head gs_sh_rotation; do
+for f in gs_capi gs_preprocess gs_binning gs_composite_fwd gs_composite_bwd gs_preprocess_bwd gs_metrics gs_losses gs_pose_loss gs_lpips gs_adapter gs_cameras gs_costvolume gs_poses gs_encoder_depth gs_gaussian_head gs_sh_rotation gs_optimizer; do
   stale=0
   for dep in "$f.cu" gs_common.cuh gs_bin_policy.h gs_det.cuh gs_tile_sort.cuh gs_inverse.cuh gs_adapter_math.cuh gs_sh_fit.h ../../include/gsplat_b200.h build.sh; do
     if [ ! -f "$f.o" ] || [ "$dep" -nt "$f.o" ]; then stale=1; fi

@@ -9,6 +9,10 @@ import subprocess
 import pytest
 import torch
 
+from tests.regimes import (DEPTH_PATTERNS, DESIGNED_CASES, PARKED, _at_pixels, designed_case, designed_depths,
+                           designed_tile_of, designed_tiles)
+from tests.sync_free_layout import regions
+
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 HEADER = os.path.join(ROOT, "include", "gsplat_b200.h")
 
@@ -39,23 +43,24 @@ def test_the_workspace_struct_layout_matches_the_header(capi, tmp_path):
     assert out[6] == capi.ABI_VERSION == 5
 
 
-def _align(x):
-    return (x + 255) // 256 * 256
-
-
 def expected_bytes(S, V, P, H, W, cap, det, cam):
-    """The layout of gs_capi.cu's sf_layout, restated: status | saved planes | list | max(forward scratch, backward)."""
-    n, ntiles = V * P, -(-W // 16) * -(-H // 16)
-    nvt, px, cap1 = V * ntiles, V * H * W, max(cap, 1)
-    status = 256
-    saved = 3 * _align(n * 16) + _align(n) + _align(nvt * 8) + 2 * _align(px * 4) + _align(8)
-    lst = _align(cap1 * 4)
-    ctr = nvt * 8 * 8 * 4                      # BIN_SUB sub-counters per tile, one per 32-byte sector
-    fwd = _align(n * 8) + 2 * _align(ctr) + _align(nvt * 8 * 4) + 2 * _align(nvt * 4) + 2 * _align(cap1 * 8)
-    warps = -(-P // 128) * 4                   # preprocess-backward warps of one scene
-    acc = n * (10 * 3 * 8 + 4) if det else n * 10 * 4
-    bwd = _align(acc) + max(warps * V * 32 * 4 if cam else 0, V * warps * 4 * 4 if det else 0)
-    return status + saved + lst + max(fwd, bwd)
+    """The layout of gs_capi.cu's sf_layout, restated region by region (tests/sync_free_layout.py, whose offsets the
+    GPU tests read the tile lists at): status | saved planes | list | max(forward scratch, backward)."""
+    return regions(S, V, P, H, W, cap, det, cam)["total"][1]
+
+
+def test_the_restated_regions_are_aligned_and_disjoint():
+    for S, V, P, H, W, cap in SHAPES:
+        for det in (False, True):
+            reg = regions(S, V, P, H, W, cap, det, True)
+            fwd = [(o, n, k) for k, (o, n) in reg.items() if k not in ("total", "backward")]
+            assert [k for _, _, k in fwd] == ["status", "rec0", "rec1", "rec2", "meta", "ranges", "final_T", "n_contrib",
+                                              "sched", "point_list", "rects", "tile_counts", "cursor", "sub_offsets",
+                                              "tile_start", "tile_n", "bucket", "tmp"]
+            for (o0, n0, k0), (o1, _, _) in zip(fwd, fwd[1:]):
+                assert o0 % 256 == 0 and o0 + n0 <= o1, k0
+            assert reg["backward"][0] == reg["rects"][0]          # the backward reuses the forward's scratch
+            assert reg["total"][1] >= max(o + n for o, n, _ in fwd)
 
 
 SHAPES = [(1, 1, 0, 1, 1, 0), (1, 1, 1, 16, 16, 1), (2, 8, 1000, 37, 53, 12345), (14, 42, 131072, 256, 256, 9_000_000),
@@ -162,3 +167,46 @@ def test_entry_points_take_a_workspace_keyword(capi):
         p = inspect.signature(fn).parameters["workspace"]
         assert p.default is None, fn
     assert inspect.signature(rasterize_batch).parameters["workspace"].kind is inspect.Parameter.KEYWORD_ONLY
+
+
+@pytest.mark.parametrize("name", DESIGNED_CASES)
+def test_designed_splats_lie_in_their_tiles(name):
+    """Every splat of a designed case (tests/regimes.py: designed_tiles) covers its designated (view, tile) and no other
+    tile, by an fp64 restatement of the projection and the 3-sigma rect with a 1 px margin, and is culled in the other
+    view: the GPU tests' exact per-tile lengths and D follow from the design."""
+    h, w, views, cells = designed_case(name)
+    d = designed_tiles(h, w, cells)
+    got = designed_tile_of(d, views)
+    want = torch.full_like(got, -1)
+    want[torch.arange(got.shape[0]), d.view] = d.tile
+    bad = (got != want).any(-1).nonzero().flatten()
+    assert bad.numel() == 0, [(int(k), got[k].tolist(), want[k].tolist()) for k in bad[:8]]
+    assert sum(d.lengths.values()) == d.means.shape[0] == sum(c[3] for c in cells)
+    # the parking spot is in front of neither camera
+    parked = designed_tiles(h, w, [(0, 0, 0, 1, "random")])
+    parked.means = torch.tensor([PARKED])
+    assert (designed_tile_of(parked, 2) == -1).all()
+
+
+def test_the_tile_restatement_sees_a_splat_near_an_edge():
+    d = designed_tiles(32, 32, [(0, 0, 0, 3, "random")])
+    d.means[1] = _at_pixels(torch.tensor(14.5), torch.tensor(6.0), torch.tensor(4.0), 32, 32)   # 1.5 px from tile 1
+    d.means[2] = _at_pixels(torch.tensor(6.0), torch.tensor(6.0), torch.tensor(0.15), 32, 32)   # before the near plane
+    assert designed_tile_of(d, 1)[:, 0].tolist() == [0, -2, -1]
+
+
+@pytest.mark.parametrize("pattern", DEPTH_PATTERNS)
+def test_designed_depth_patterns(pattern):
+    """Each pattern is in its regime as built; the GPU tests assert the same of the device's own depths."""
+    z = designed_depths(pattern, 8193, torch.Generator().manual_seed(0))
+    bits = z.view(torch.int32).long() & 0xffffffff
+    distinct = bits.unique().numel()
+    if pattern == "equal":
+        assert distinct == 1
+    elif pattern == "ulp":
+        assert distinct >= 256 and (bits >> 16).unique().numel() == 1
+    elif pattern == "binades":
+        assert all(((bits >> (8 * k)) & 255).unique().numel() > 1 for k in range(4))
+    elif pattern == "reversed":
+        assert (z[1:] < z[:-1]).all()
+    assert (z > 0.2).all()
